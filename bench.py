@@ -6,7 +6,7 @@ Config (BASELINE.json "headline"): ``zigzag_ring_flash_attn_qkvpacked_func``, bf
 (strong scaling: 32768/N tokens per GPU, total attention work constant).  One step = forward + backward of
 the attention op through the public API.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--config readme]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--config readme] [--dump-outputs DIR]
 
 ``--impl reference`` runs the unmodified zhuzilin/ring-flash-attention installed in ``baseline/_ref``
 (flash_attn 2.8 + NCCL) on the same config and prints the same JSON line with ``"impl": "reference"``.
@@ -18,6 +18,11 @@ barrier + synchronize on both sides of the timed region, max over ranks.  ``e2e`
 with the step's inputs copied from pinned host memory and the loss read back every step; the copy of step i+1 is
 prefetched on a side stream into a double buffer while step i computes (same loop for both arms,
 ``RFA_BENCH_E2E_PREFETCH=0`` serialises copy and compute again).
+
+``--dump-outputs DIR`` writes what the last timed step returned to its caller (rank 0): ``out`` and, for fwd_bwd,
+the gradient of every input, as float32 ``DIR/<name>.npy``.  The inputs are seeded, so two builds run with the same
+arguments can be compared output for output; each array is a fixed, seeded sample of DUMP_ROWS token rows (all
+heads and head dims) so that the files stay small at the benchmark shape.
 """
 from __future__ import annotations
 
@@ -49,7 +54,28 @@ def parse():
     ap.add_argument("--check", dest="check", action="store_true", default=True,
                     help="verify one untimed step against the fp32 oracle on sampled rows (default: on, ours only)")
     ap.add_argument("--no-check", dest="check", action="store_false")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (sampled token rows) as float32 DIR/<name>.npy")
     return ap.parse_args()
+
+
+DUMP_ROWS = 512  # token rows per dumped array: out + dqkv at the headline shape are 32 MiB in all
+
+
+def dump_outputs(torch, dir_, api, out, dev_in, tokens):
+    """Seeded sample of the token rows of ``out`` and of every input gradient, as float32 .npy files."""
+    import numpy as np
+
+    os.makedirs(dir_, exist_ok=True)
+    g = torch.Generator().manual_seed(0)
+    rows = torch.randperm(tokens, generator=g)[:min(DUMP_ROWS, tokens)].sort().values.to(out.device)
+    arrays = {"out": out}
+    names = ["qkv"] if api == "qkvpacked" else ["q", "kv"]
+    for name, t in zip(names, dev_in):
+        if t.grad is not None:
+            arrays[f"grad_{name}"] = t.grad
+    for name, t in arrays.items():
+        np.save(os.path.join(dir_, f"{name}.npy"), t.detach()[0].index_select(0, rows).float().cpu().numpy())
 
 
 class ClockSampler:
@@ -248,14 +274,18 @@ def main():
     loss_host = torch.zeros(1, dtype=torch.float32).pin_memory()
     h2d_bytes = sum(t.numel() * t.element_size() for t in host_in)
 
+    last = {}
+
     def step(inputs):
         if args.mode == "fwd":
             with torch.no_grad():
-                return fn(*inputs, causal=True)
+                last["out"] = fn(*inputs, causal=True)
+            return last["out"]
         for t in inputs:
             t.grad = None
         out = fn(*inputs, causal=True)
         out.backward(dout)
+        last["out"] = out
         return out
 
     def e2e_step():
@@ -313,6 +343,8 @@ def main():
     step_stats = dict(stats)
     if args.impl == "ours":
         launches = counter.value
+    if args.dump_outputs and rank == 0:
+        dump_outputs(torch, args.dump_outputs, api, last["out"], dev_in, tokens)
     e2e = None
     if not args.no_e2e:
         pipeline = "serial copy -> compute"

@@ -9,8 +9,9 @@
   stripe8 : stripe_flash_attn_qkvpacked_func              block-scaled fp8 inputs, bs=2 seq=16384 nheads=16
 
 Every line carries the achieved fraction of the path's roofline: the slower of (attention FLOPs of one rank at
-the measured sustained bf16 GEMM rate, MEASURED_PEAKS.json) and (bytes the rank must receive over NVLink at the
-measured peer-copy bandwidth).  Timing: CUDA events per step, L2 flushed between steps, max over ranks.
+the H100 SXM data-sheet dense bf16 rate) and (bytes the rank must receive over NVLink at the data-sheet NVLink 4
+bandwidth per direction).  Both are data-sheet figures for a 700 W card, not measured rates; a card with a lower
+power limit or lower clocks will not reach them.  Timing: CUDA events per step, L2 flushed between steps, max over ranks.
 The reference has no fp8 entry point, so ``stripe8`` runs its bf16 function on the dequantised tensors.
 """
 from __future__ import annotations
@@ -25,15 +26,8 @@ import torch.distributed as dist
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-NVLINK_GBS = 770.0  # measured peer copy, one direction (B200_PROFILING.md)
-
-
-def peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return float(json.load(f)["bf16_tflops_sustained"])
-    except (OSError, KeyError, ValueError):
-        return 1412.2
+NVLINK_GBS = 450.0  # NVLink 4 per direction per GPU, H100 SXM data sheet (not a measured rate)
+BF16_TFLOPS = 989.0  # dense bf16 tensor-core rate, H100 SXM data sheet at 700 W (not a measured rate)
 
 
 def causal_flops(doc_lens, hq, d, fwd_only):
@@ -129,7 +123,7 @@ def main():
     def report(name, api, ms, med, flops_rank, rx_bytes, extra):
         if rank != 0:
             return
-        t_flops = flops_rank / (peaks() * 1e12) * 1e3
+        t_flops = flops_rank / (BF16_TFLOPS * 1e12) * 1e3
         t_link = rx_bytes / (NVLINK_GBS * 1e9) * 1e3
         bound = max(t_flops, t_link)
         print(json.dumps({
@@ -137,7 +131,7 @@ def main():
             "mode": "fwd" if args.forward_only else "fwd_bwd", "ms_per_step": ms, "ms_median": med,
             "iter_per_s": 1000.0 / ms, "tflops_per_gpu": flops_rank / (ms * 1e-3) / 1e12,
             "roofline": {"compute_ms": t_flops, "nvlink_ms": t_link, "bound": "compute" if t_flops >= t_link else "nvlink",
-                         "fraction": bound / ms},
+                         "fraction": bound / ms, "peaks": "H100 SXM data sheet (989 TFLOP/s bf16, 450 GB/s NVLink)"},
             "steps": args.steps, "warmup": args.warmup, "l2": "flushed between steps", **extra}), flush=True)
 
     fwd = args.forward_only

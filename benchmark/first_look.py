@@ -1,4 +1,4 @@
-"""Single-GPU kernel timings: sm_100a kernels vs flash_attn 2.8 (the kernel the reference calls)."""
+"""Single-GPU kernel timings: sm_90a kernels vs flash_attn 2.8 (the kernel the reference calls)."""
 import json
 import os
 import sys

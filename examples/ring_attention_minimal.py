@@ -6,7 +6,7 @@ full qkv, cut out this rank's shard by hand, compare with single-device flash at
 with the hand-written slicing replaced by ``parallel.layouts`` and the printed differences by an assertion.
 
     torchrun --nproc-per-node 2 examples/ring_attention_minimal.py                  # CPU, gloo
-    torchrun --nproc-per-node 8 examples/ring_attention_minimal.py --cuda           # B200s, fused NVLink path
+    torchrun --nproc-per-node 8 examples/ring_attention_minimal.py --cuda           # H100s, fused NVLink path
     torchrun --nproc-per-node 8 examples/ring_attention_minimal.py --cuda --scheme stripe --seqlen 65536
 """
 import argparse

@@ -4,7 +4,7 @@
 The flow is the one the reference documents for its adapter (/root/reference/README.md:35-61,
 ring_flash_attn/adapters/hf_adapter.py): patch transformers once, publish the batch's global ``cu_seqlens`` once
 per step, then feed every rank its contiguous slice of the token stream.  Runs on CPU/gloo (dense fp32 blocks) or
-on GPUs (sm_100a kernels, fused NVLink path):
+on GPUs (sm_90a kernels, fused NVLink path):
 
     torchrun --nproc-per-node 2 examples/train_hf_llama_cp.py            # CPU, gloo
     torchrun --nproc-per-node 8 examples/train_hf_llama_cp.py --cuda     # one process per GPU

@@ -1,4 +1,4 @@
-"""ring_flash_attn_b200 - Blackwell-native context-parallel flash attention.
+"""ring_flash_attn_b200 - Hopper-native context-parallel flash attention.
 
 Public surface mirrors zhuzilin/ring-flash-attention (/root/reference/ring_flash_attn/__init__.py:1-35).
 The Hugging Face adapter is imported lazily so that ``import ring_flash_attn_b200`` never requires

@@ -1,4 +1,4 @@
-"""In-tree build of ``ring_flash_attn_b200/_C*.so`` for sm_100a.
+"""In-tree build of ``ring_flash_attn_b200/_C*.so`` for sm_90a (H100).
 
 nvcc cross-compiles without a GPU, so this runs on the CPU dev box; the resulting shared object lives
 next to the sources (git-ignored) and travels with the tree.  Incremental: a translation unit is rebuilt
@@ -16,12 +16,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-DRFA_BUILD"]
 if os.environ.get("RFA_TRACE", "0") == "1":
     NVCC_FLAGS.append("-DRFA_TRACE")
-CU_SOURCES = ["attn_fwd_sm100.cu", "attn_bwd_sm100.cu", "tensor_map.cu", "lse_layout.cu", "probe_sm100.cu",
-              "probe_fp8_sm100.cu", "comm_sm100.cu"]
+CU_SOURCES = ["attn_fwd_sm90.cu", "attn_bwd_sm90.cu", "tensor_map.cu", "lse_layout.cu", "comm_sm90.cu"]
 CPP_SOURCES = ["bindings.cpp", "peer_mem.cpp"]
 
 

@@ -1,4 +1,4 @@
-// Host/device shared structures for the sm_100a attention kernels.
+// Host/device shared structures for the sm_90a attention kernels.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -8,10 +8,10 @@ namespace rfa {
 
 constexpr int kDiagFull = 1 << 29;  // "no causal boundary": every key of the segment is visible
 
-// One CTA work item: up to 256 consecutive query rows of one query chunk (two 128-row MMA tiles).
+// One CTA work item: up to 128 consecutive query rows of one query chunk (two 64-row wgmma tiles).
 struct alignas(16) WorkItem {
   int q_row0;     // first local query row
-  int q_rows;     // 1..256
+  int q_rows;     // 1..128
   int q_off;      // offset of q_row0 inside its chunk (the diagonal is expressed in chunk rows)
   int seg_begin;  // first entry in the segment table
   int seg_count;
@@ -107,7 +107,7 @@ struct DkvParams {
   int my_rank;
 };
 
-// Owner-side reduction of the inbox (model dtype partials, summed in fp32) into dK / dV (csrc/comm_sm100.cu).
+// Owner-side reduction of the inbox (model dtype partials, summed in fp32) into dK / dV (csrc/comm_sm90.cu).
 struct alignas(16) ReduceTask {
   int row0, rows;
   unsigned src_mask;  // ranks whose slot holds a partial for these rows
@@ -148,9 +148,8 @@ struct FwdParams {
   const float* v_ref;
   int q_scale_block, kv_scale_block;
   long long kv_scale_row0;
-  int flags;  // tuning / timing switches (RFA_B200_FWD_FLAGS): bit 0 = no turn-taking between the two softmax
-              // warpgroups; bit 1 = do not wait for remote K/V (compute-only timing, wrong numbers); bit 2 = no
-              // compute (communication-only timing)
+  int flags;  // timing switches (RFA_B200_FWD_FLAGS): bit 1 = do not wait for remote K/V (compute-only timing,
+              // wrong numbers); bit 2 = no compute (communication-only timing)
   void* out;  // (rows, hq, 128) contiguous, input dtype
   float* lse;  // index = (row / lse_S) * hq * lse_S + head * lse_S + row % lse_S
   int lse_S;
@@ -209,17 +208,6 @@ struct BwdParams {
   DkvParams dkv;
 };
 
-// Descriptor probe (csrc/probe_sm100.cu): operand forms + optional run-time overrides (-1 = kernel default).
-struct ProbeConfig {
-  int a_kind, b_kind;
-  int n;     // 128 or 64
-  int kdim;  // 128 or 64
-  int lbo_a, sbo_a, kstep_a;
-  int lbo_b, sbo_b, kstep_b;
-  int reps;                 // > 1: repeat the k-loop to measure MMA throughput
-  unsigned long long* cycles;  // optional: elapsed SM cycles of the issue-to-completion window
-};
-
 // dtype codes shared with the Python side
 enum : int { kDtypeBF16 = 0, kDtypeFP16 = 1, kDtypeE4M3 = 2 };
 
@@ -234,10 +222,6 @@ const char* attn_bwd_delta_launch(int dtype, const TensorView& out, const Tensor
 const char* attn_bwd_launch(int dtype, const TensorView& q, const TensorView& dout, const TensorView& k,
                             const TensorView& v, const TensorView& k_stage, const TensorView& v_stage,
                             const TensorView& dq_accum, const BwdParams& p, cudaStream_t stream);
-const char* probe_launch(const TensorView& a, const TensorView& b, const void* a_raw, const void* b_raw, float* out,
-                         const ProbeConfig& c, cudaStream_t stream);
-const char* probe_fp8_launch(const TensorView& a, const TensorView& b, float* out, const ProbeConfig& c,
-                             cudaStream_t stream);
 const char* lse_flatten_launch(const float* in, float* out, const int* cu, int batch, int heads, int max_seqlen,
                                int total, cudaStream_t stream);
 const char* lse_unflatten_launch(const float* in, float* out, const int* cu, int batch, int heads, int max_seqlen,

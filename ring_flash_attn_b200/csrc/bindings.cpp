@@ -1,4 +1,4 @@
-// Python bindings for the sm_100a kernels and the peer-memory runtime (module ring_flash_attn_b200._C).
+// Python bindings for the sm_90a kernels and the peer-memory runtime (module ring_flash_attn_b200._C).
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -15,13 +15,13 @@ using rfa::TensorView;
 int dtype_code(const at::Tensor& t) {
   if (t.scalar_type() == at::kBFloat16) return rfa::kDtypeBF16;
   if (t.scalar_type() == at::kHalf) return rfa::kDtypeFP16;
-  TORCH_CHECK(false, "ring_flash_attn_b200: only bf16 / fp16 inputs are supported by the sm_100a kernels");
+  TORCH_CHECK(false, "ring_flash_attn_b200: only bf16 / fp16 inputs are supported by the sm_90a kernels");
 }
 
 TensorView view3(const at::Tensor& t, const char* name) {
   TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor");
   TORCH_CHECK(t.dim() == 3, name, " must be (rows, heads, head_dim)");
-  TORCH_CHECK(t.size(2) == 128 || t.size(2) == 64, name, ": the sm_100a kernels are instantiated for head_dim 64 and 128");
+  TORCH_CHECK(t.size(2) == 128 || t.size(2) == 64, name, ": the sm_90a kernels are instantiated for head_dim 64 and 128");
   TORCH_CHECK(t.stride(2) == 1, name, ": last dimension must be contiguous");
   return TensorView{t.data_ptr(), t.size(0), static_cast<int>(t.size(1)), t.stride(0), t.stride(1)};
 }
@@ -336,7 +336,7 @@ void attn_bwd_fused_window(const at::Tensor& q, const at::Tensor& dout, const at
                 true);
 }
 
-// Owner-side reduction of the dK/dV inbox (csrc/comm_sm100.cu).
+// Owner-side reduction of the dK/dV inbox (csrc/comm_sm90.cu).
 void reduce_dkv(const at::Tensor& inbox, int64_t slot_stride, int64_t kv_stride, at::Tensor& dk, at::Tensor& dv,
                 const at::Tensor& tasks, const FusedCtx& fc, int64_t ticket_target) {
   const c10::cuda::CUDAGuard guard(inbox.device());
@@ -362,60 +362,13 @@ void reduce_dkv(const at::Tensor& inbox, int64_t slot_stride, int64_t kv_stride,
   check(rfa::reduce_dkv_launch(dtype_code(dk), p, at::cuda::getCurrentCUDAStream()));
 }
 
-// dq = cast(acc); acc = 0  (csrc/comm_sm100.cu: dq_finalize_kernel)
+// dq = cast(acc); acc = 0  (csrc/comm_sm90.cu: dq_finalize_kernel)
 void dq_finalize(at::Tensor& acc, at::Tensor& out) {
   const c10::cuda::CUDAGuard guard(acc.device());
   TORCH_CHECK(acc.scalar_type() == at::kFloat && acc.is_contiguous() && out.is_contiguous() &&
               acc.numel() == out.numel());
   check(rfa::dq_finalize_launch(dtype_code(out), acc.data_ptr<float>(), out.data_ptr(), acc.numel(),
                                 at::cuda::getCurrentCUDAStream()));
-}
-
-// kind::f8f6f4 descriptor probe (csrc/probe_fp8_sm100.cu): a, b are (128, 128) float8_e4m3fn tensors;
-// cfg = {a_kind (0 smem K-major, 1 TMEM), b_kind (0 K-major, 1 MN-major), tmem byte order, lbo_b, sbo_b, kstep_b}
-at::Tensor probe_fp8(const at::Tensor& a, const at::Tensor& b, std::vector<int64_t> cfg) {
-  const c10::cuda::CUDAGuard guard(a.device());
-  TORCH_CHECK(cfg.size() == 6);
-  TORCH_CHECK(a.is_contiguous() && b.is_contiguous() && a.element_size() == 1 && b.element_size() == 1 &&
-              a.numel() == 128 * 128 && b.numel() == 128 * 128);
-  rfa::ProbeConfig c{};
-  c.a_kind = static_cast<int>(cfg[0]);
-  c.b_kind = static_cast<int>(cfg[1]);
-  c.n = 128;
-  c.kdim = 128;
-  c.lbo_a = static_cast<int>(cfg[2]);
-  c.sbo_a = c.kstep_a = -1;
-  c.lbo_b = static_cast<int>(cfg[3]);
-  c.sbo_b = static_cast<int>(cfg[4]);
-  c.kstep_b = static_cast<int>(cfg[5]);
-  c.reps = 1;
-  c.cycles = nullptr;
-  TensorView va{a.data_ptr(), 128, 1, 128, 128}, vb{b.data_ptr(), 128, 1, 128, 128};
-  at::Tensor out = at::zeros({128, 128}, a.options().dtype(at::kFloat));
-  check(rfa::probe_fp8_launch(va, vb, out.data_ptr<float>(), c, at::cuda::getCurrentCUDAStream()));
-  return out;
-}
-
-at::Tensor probe(const at::Tensor& a, const at::Tensor& b, std::vector<int64_t> cfg) {
-  // a: (rows, 128) or (128, kdim) bf16 ; b likewise; cfg = {a_kind, b_kind, n, kdim, lbo_a, sbo_a, kstep_a, lbo_b, sbo_b, kstep_b}
-  const c10::cuda::CUDAGuard guard(a.device());
-  TORCH_CHECK(cfg.size() == 10 || cfg.size() == 11);
-  rfa::ProbeConfig c{static_cast<int>(cfg[0]), static_cast<int>(cfg[1]), static_cast<int>(cfg[2]),
-                     static_cast<int>(cfg[3]), static_cast<int>(cfg[4]), static_cast<int>(cfg[5]),
-                     static_cast<int>(cfg[6]), static_cast<int>(cfg[7]), static_cast<int>(cfg[8]),
-                     static_cast<int>(cfg[9]), cfg.size() == 11 ? static_cast<int>(cfg[10]) : 1, nullptr};
-  at::Tensor cyc = at::zeros({2}, a.options().dtype(at::kLong));
-  c.cycles = reinterpret_cast<unsigned long long*>(cyc.data_ptr());
-  TORCH_CHECK(a.is_contiguous() && b.is_contiguous() && a.scalar_type() == at::kBFloat16 &&
-              b.scalar_type() == at::kBFloat16);
-  TensorView va{nullptr, 0, 1, 128, 128}, vb{nullptr, 0, 1, 128, 128};
-  if (c.a_kind == 0 || c.a_kind == 3) va = TensorView{a.data_ptr(), a.size(0), 1, 128, 128};
-  if (c.b_kind == 0 || c.b_kind == 1) vb = TensorView{b.data_ptr(), b.size(0), 1, 128, 128};
-  at::Tensor out = at::zeros({128, c.n}, a.options().dtype(at::kFloat));
-  check(rfa::probe_launch(va, vb, a.data_ptr(), b.data_ptr(), out.data_ptr<float>(), c,
-                          at::cuda::getCurrentCUDAStream()));
-  if (cfg.size() == 11) return cyc;  // throughput mode: (total cycles, issue cycles)
-  return out;
 }
 
 at::Tensor lse_flatten(const at::Tensor& lse, const at::Tensor& cu) {
@@ -446,7 +399,7 @@ at::Tensor lse_unflatten(const at::Tensor& lse, const at::Tensor& cu, int64_t ma
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "ring_flash_attn_b200 sm_100a kernels";
+  m.doc() = "ring_flash_attn_b200 sm_90a kernels";
   pybind11::class_<FusedCtx>(m, "FusedCtx")
       .def(pybind11::init<>())
       .def_readwrite("k_stage", &FusedCtx::k_stage)
@@ -488,8 +441,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("dq_finalize", &dq_finalize);
   m.def("attn_bwd_delta", &attn_bwd_delta);
   m.def("attn_bwd", &attn_bwd);
-  m.def("probe", &probe);
-  m.def("probe_fp8", &probe_fp8);
   m.def("lse_flatten", &lse_flatten);
   m.def("lse_unflatten", &lse_unflatten);
   rfa::bind_peer_mem(m);

@@ -17,7 +17,7 @@
 #include <cstdlib>
 
 #include "attn_common.h"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace rfa {
 
@@ -38,18 +38,13 @@ inline void set_peer_timeout_from_env() {
 __device__ __forceinline__ bool epoch_reached(uint32_t have, uint32_t want) {
   return static_cast<int32_t>(have - want) >= 0;
 }
-__device__ __forceinline__ void wait_epoch(const uint32_t* flag, uint32_t want, const char* what, int who = -1,
-                                           int idx = -1) {
+// Traps (without a message, see RFA_WATCHDOG_NS in sm90_ptx.cuh) after RFA_B200_PEER_TIMEOUT_S; 0 disables the limit.
+__device__ __forceinline__ void wait_epoch(const uint32_t* flag, uint32_t want) {
   if (epoch_reached(ld_acquire_sys(flag), want)) return;
   const uint64_t t0 = global_timer_ns();
   const unsigned long long limit = g_peer_timeout_ns;
   while (!epoch_reached(ld_acquire_sys(flag), want)) {
-    if (limit != 0 && global_timer_ns() - t0 > limit) {
-      printf("rfa: gave up waiting for a peer after %llu s (%s) rank %d peer/flag %d block %d want %u have %u "
-             "(RFA_B200_PEER_TIMEOUT_S raises the limit, 0 disables it)\n", limit / 1000000000ull, what, who, idx,
-             blockIdx.x, want, ld_acquire_sys(flag));
-      __trap();
-    }
+    if (limit != 0 && global_timer_ns() - t0 > limit) __trap();
     __nanosleep(64);  // the peer is microseconds to seconds away: do not hammer the memory system while spinning
   }
 }
@@ -97,7 +92,7 @@ __device__ __forceinline__ void push_role(const PushParams& pp) {
     const PushTask t = push_task_at(pp, ti);
     if (tid == 0 && pp.epoch > 2 && t.rows > 0) {
       // the destination must have finished reading what we pushed into this staging parity two calls ago
-      wait_epoch(pp.my_pad + kPadConsumed + t.dst, pp.epoch - 2, "staging reuse", pp.my_rank, t.dst);
+      wait_epoch(pp.my_pad + kPadConsumed + t.dst, pp.epoch - 2);
     }
     __syncthreads();
     const int vec_per_row = pp.row_bytes >> 4;
@@ -170,9 +165,8 @@ __device__ __forceinline__ void push_role_tma(const PushParams& pp, uint8_t* sme
   uint32_t n_loaded = 0, n_stored = 0;  // global piece counters (ring position / parity)
   // Completion is published per DESTINATION, not per task: the tasks of a CTA are sorted by destination, so the
   // copy pipeline keeps running across task boundaries and is drained (all bytes written, system-scope fence)
-  // only when the destination changes.  Round 1 drained after every 512 KB task - a load-latency fill plus an
-  // NVLink write-completion wait per task, which at 8 GPUs (28 tasks per CTA) held the push to ~290 GB/s per GPU
-  // (profiles/r2/trip_diag8_compute_vs_comm.log).
+  // only when the destination changes: draining after every task would cost a load-latency fill plus an NVLink
+  // write-completion wait per task.
   int cur_dst = -1;
   uint32_t pending = 0;  // finished tasks for cur_dst that are not yet counted
   auto publish = [&]() {
@@ -194,7 +188,7 @@ __device__ __forceinline__ void push_role_tma(const PushParams& pp, uint8_t* sme
       cur_dst = t.dst;
     }
     if (pp.epoch > 2 && t.rows > 0)
-      wait_epoch(pp.my_pad + kPadConsumed + t.dst, pp.epoch - 2, "staging reuse", pp.my_rank, t.dst);
+      wait_epoch(pp.my_pad + kPadConsumed + t.dst, pp.epoch - 2);
     const long long pitch = pp.src_row_bytes[t.which];
     const char* src = pp.src_base[t.which] + t.src_row * pitch;
     char* dst = pp.stage_ptrs[t.dst] + pp.parity_off + t.dst_off;

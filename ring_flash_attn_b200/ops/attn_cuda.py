@@ -1,6 +1,6 @@
-"""Python side of the sm_100a attention kernels: plan -> device work tables -> launches.
+"""Python side of the sm_90a attention kernels: plan -> device work tables -> launches.
 
-The kernels (``csrc/attn_fwd_sm100.cu`` / ``attn_bwd_sm100.cu``) consume a :class:`CPPlan` as two small
+The kernels (``csrc/attn_fwd_sm90.cu`` / ``attn_bwd_sm90.cu``) consume a :class:`CPPlan` as two small
 int32 tables.  Tables are cached on the plan object (plans themselves are lru-cached per shape), so the
 steady state of a training loop performs no host work beyond the launches.
 
@@ -22,7 +22,7 @@ from . import cuda_ext
 from .plan import CPPlan, Segment
 
 DIAG_FULL = 1 << 29
-Q_ITEM_ROWS = 256  # rows per forward CTA (two 128-row MMA tiles)
+Q_ITEM_ROWS = 128  # rows per forward CTA (two 64-row wgmma tiles)
 K_TILE_ROWS = 128  # keys per backward CTA
 
 
@@ -121,9 +121,8 @@ def has_window(segs: Sequence[Segment]) -> bool:
 
 
 def window_kernels_enabled() -> bool:
-    """Sliding-window plans run on the kWindow kernel variants (validated on B200 in round 2:
-    profiles/r2/trip_single_variants.log, trip_multi2_bulk_configs.log).  ``RFA_B200_WINDOW_KERNEL=0`` forces the
-    dense torch blocks (``parallel/engine.py``) for debugging."""
+    """Sliding-window plans run on the kWindow kernel variants.  ``RFA_B200_WINDOW_KERNEL=0`` forces the dense torch
+    blocks (``parallel/engine.py``) for debugging."""
     import os
 
     return os.environ.get("RFA_B200_WINDOW_KERNEL", "1") != "0"
@@ -166,7 +165,7 @@ def fwd_tables_window_host(plan: CPPlan, segs: Sequence[Segment], row_offset: Di
                            flag_of_src: Optional[Dict[int, int]] = None):
     """Forward tables for sliding-window plans: (items, segments, seg_lo, all_rows_covered).
 
-    Key j of a segment is visible to chunk row i iff ``i + lo <= j <= i + diag``.  Every work item (256 query
+    Key j of a segment is visible to chunk row i iff ``i + lo <= j <= i + diag``.  Every work item (128 query
     rows starting at chunk row ``off``) gets its OWN copy of each segment, trimmed at the front to the first key
     its first row can see (``off + lo``): the kernel's key loop then still starts at tile 0 and only has to mask
     the slanted lower edge, for which ``seg_lo`` carries the re-based offset."""
@@ -369,7 +368,7 @@ def bwd_tables_fused(plan: CPPlan, row_offset: Dict[int, int], device, flag_of_s
 
 class _DqWorkspace:
     """fp32 dQ accumulators, one per (device, stream, element count), kept ZEROED between calls: the backward
-    kernel adds its partial tiles into it and ``dq_finalize`` (csrc/comm_sm100.cu) writes the model-dtype result and
+    kernel adds its partial tiles into it and ``dq_finalize`` (csrc/comm_sm90.cu) writes the model-dtype result and
     zeroes the accumulator again in the same pass.  Replaces a ``torch.zeros`` before and a ``.to(dtype)`` after
     every backward (the reference's fp32 dq bookkeeping: /root/reference/ring_flash_attn/ring_flash_attn.py:134-154)."""
 

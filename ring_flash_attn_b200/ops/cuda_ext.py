@@ -1,8 +1,8 @@
-"""Loader for the in-tree sm_100a extension (``ring_flash_attn_b200/_C*.so``).
+"""Loader for the in-tree sm_90a extension (``ring_flash_attn_b200/_C*.so``).
 
 The extension is built ahead of time by ``__graft_entry__.build()`` / ``python setup.py build_ext
 --inplace`` (nvcc cross-compiles without a GPU) so that it travels with the source tree.  On a
-Blackwell GPU a missing extension is a hard error - the CUDA path must never silently fall back.
+Hopper GPU a missing extension is a hard error - the CUDA path must never silently fall back.
 """
 from __future__ import annotations
 
@@ -14,9 +14,9 @@ import torch
 
 
 @functools.lru_cache(maxsize=None)
-def _device_is_sm100(index: int) -> bool:
+def _device_is_sm90(index: int) -> bool:
     major, _minor = torch.cuda.get_device_capability(index)
-    return major == 10
+    return major == 9
 
 
 @functools.lru_cache(maxsize=None)
@@ -25,16 +25,16 @@ def load():
         return importlib.import_module("ring_flash_attn_b200._C")
     except ImportError as e:  # pragma: no cover - exercised only on broken installs
         raise RuntimeError(
-            "ring_flash_attn_b200._C (the sm_100a extension) is not built; run "
+            "ring_flash_attn_b200._C (the sm_90a extension) is not built; run "
             "`python -c 'import __graft_entry__ as g; g.build()'` or `python setup.py build_ext --inplace`"
         ) from e
 
 
 def available_for(t: torch.Tensor) -> bool:
-    """True when ``t`` lives on a Blackwell GPU (then the extension is mandatory)."""
+    """True when ``t`` lives on a Hopper GPU (then the extension is mandatory)."""
     if not t.is_cuda or os.environ.get("RFA_B200_FORCE_TORCH", "0") == "1":
         return False
-    if not _device_is_sm100(t.device.index if t.device.index is not None else torch.cuda.current_device()):
+    if not _device_is_sm90(t.device.index if t.device.index is not None else torch.cuda.current_device()):
         return False
     load()
     return True

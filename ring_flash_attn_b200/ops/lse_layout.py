@@ -3,7 +3,7 @@
 Parity with the reference's ``flatten_varlen_lse`` / ``unflatten_varlen_lse`` (TorchScript:
 /root/reference/ring_flash_attn/utils.py:76-95; Triton kernels: triton_utils.py:6-137): convert
 between the padded ``(batch, H, max_seqlen)`` layout of old flash-attn and the packed ``(H, total)``
-layout.  On CUDA the work is done by the small sm_100a copy kernels in ``csrc/lse_layout.cu``; on CPU
+layout.  On CUDA the work is done by the small sm_90a copy kernels in ``csrc/lse_layout.cu``; on CPU
 (and as the oracle for the kernels) by the torch implementation below.
 """
 from __future__ import annotations

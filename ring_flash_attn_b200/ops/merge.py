@@ -1,7 +1,7 @@
 """Online-softmax merge of partial attention results.
 
 Capability parity with the reference's ``update_out_and_lse`` (/root/reference/ring_flash_attn/utils.py:32-73).
-The fused sm_100a path never calls this - the accumulator stays in tensor memory across key
+The fused sm_90a path never calls this - the accumulator stays in registers across key
 shards - but the torch.distributed fallback path and the tests do.
 
 Layout here is token-major: out ``(T, H, D)`` fp32, lse ``(H, T)`` fp32.  ``-inf`` lse (a row that

@@ -12,7 +12,7 @@ Every sharding scheme of the reference is a statement about *global token positi
 Instead of hand-writing a per-scheme step loop, this module turns (scheme, rank, world, shapes,
 cu_seqlens) into a *plan*: local query chunks plus, for every source rank, the key segments each
 chunk may see and the diagonal offset of the causal boundary (key ``j`` visible to query ``i`` iff
-``j <= i + diag``).  The torch fallback executes a plan with ``ops.dense.block_fwd``; the sm_100a
+``j <= i + diag``).  The torch fallback executes a plan with ``ops.dense.block_fwd``; the sm_90a
 kernels consume the very same plan as a device table and compute the masks in-kernel.
 
 Rows are token-major: a batch tensor ``(B, S_l, H, D)`` is the row range ``[b*S_l, (b+1)*S_l)``.

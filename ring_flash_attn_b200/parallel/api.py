@@ -7,7 +7,7 @@ ring_flash_attn_varlen.py:268-358, zigzag_ring_flash_attn_varlen.py:415-505,
 llama3_flash_attn_varlen.py:390-504) so a user can switch by changing the import.
 
 Unlike the reference there is a single autograd bridge: each scheme only contributes a *plan*
-(``ops/plan.py``); the engine (``parallel/engine.py``) runs it on the fused sm_100a path or on the
+(``ops/plan.py``); the engine (``parallel/engine.py``) runs it on the fused sm_90a path or on the
 torch.distributed fallback.
 """
 from __future__ import annotations
@@ -41,7 +41,7 @@ __all__ = [
 # the op: one torch.library custom op for every scheme (parallel/ops.py)
 # ----------------------------------------------------------------------------------------------
 
-KERNEL_HEAD_DIMS = (64, 128)  # the sm_100a kernels are instantiated for these head sizes
+KERNEL_HEAD_DIMS = (64, 128)  # the sm_90a kernels are instantiated for these head sizes
 KERNEL_HEAD_DIM = KERNEL_HEAD_DIMS[-1]
 
 
@@ -49,7 +49,7 @@ def _pad_head_dim(q) -> int:
     """Columns of zero padding that bring the head size to the next one the kernels are instantiated for (64, 128).
 
     Zero columns change neither Q.K^T nor the first ``d`` columns of P.V, and their gradients are exactly zero,
-    so e.g. head size 80 or 96 runs on the tcgen05 kernels as 128 (at the cost of the padded FLOPs) and 32 as 64,
+    so e.g. head size 80 or 96 runs on the wgmma kernels as 128 (at the cost of the padded FLOPs) and 32 as 64,
     instead of dropping to the dense torch blocks.  ``RFA_B200_PAD_HEAD_DIM=0`` disables it, ``=force`` applies it
     on any device (used by the CPU tests)."""
     mode = os.environ.get("RFA_B200_PAD_HEAD_DIM", "1")
@@ -150,7 +150,7 @@ def _scale_table(descale, x) -> Optional[torch.Tensor]:
 
 def _fp8_kernel_scales(q, k, v, dq, dk, dv, window_size):
     """Descale tables ``(q, k, v)`` for the fp8 forward kernel, or None when the call does not qualify: e4m3 q/k/v
-    with head_dim 128 on a Blackwell GPU, descales per tensor / head / token block x head (``_scale_table``), no
+    with head_dim 128 on a Hopper GPU, descales per tensor / head / token block x head (``_scale_table``), no
     sliding window, ``RFA_B200_FP8_KERNEL`` != 0.  Whether the K / V blocks line up with the 128-key tiles of the plan
     is decided inside the op (parallel/ops.py); anything else takes the dequantise-to-bf16 path."""
     if os.environ.get("RFA_B200_FP8_KERNEL", "2") == "0":

@@ -1,7 +1,7 @@
 """torch.distributed transports used by the fallback (CPU/gloo, or GPUs without peer access).
 
 Capability parity with the reference's ``RingComm`` and ``AllGatherComm``
-(/root/reference/ring_flash_attn/utils.py:98-168).  The fused sm_100a path does not use these: the
+(/root/reference/ring_flash_attn/utils.py:98-168).  The fused sm_90a path does not use these: the
 attention kernels' own communication CTAs push K/V rows into the peers' memory over NVLink
 (``parallel/symm.py``, ``csrc/comm_device.cuh``).
 """

@@ -2,15 +2,15 @@
 
 Two transports, selected per call:
 
-* ``fused``   - sm_100a kernels; the attention kernel's own communication CTAs push the K/V rows each
+* ``fused``   - sm_90a kernels; the attention kernel's own communication CTAs push the K/V rows each
                 peer needs into that peer's memory over NVLink, and the backward stores dK/dV partials
                 straight into the owner's inbox (``parallel/fused.py`` / ``parallel/symm.py``).  Used
-                whenever the tensors live on Blackwell GPUs of one node with peer access.
+                whenever the tensors live on Hopper GPUs of one node with peer access.
 * ``ring`` / ``allgather`` - torch.distributed fallback (gloo on CPU, NCCL on GPUs without peer
                 access): the reference's own communication pattern
                 (/root/reference/ring_flash_attn/ring_flash_attn.py:26-63,97-152 and
                 llama3_flash_attn_varlen.py:89-158,218-297) around ``ops.dense`` blocks (CPU) or the
-                single-GPU sm_100a kernel (CUDA).
+                single-GPU sm_90a kernel (CUDA).
 
 All tensors here are token-major: q ``(Tq,Hq,D)``, k/v ``(Tk,Hkv,D)``, lse ``(Hq,Tq)`` fp32.
 """
@@ -33,12 +33,12 @@ from .comm import AllGatherComm, RingComm
 # ----------------------------------------------------------------------------------------------
 
 def _use_cuda_kernels(q: torch.Tensor, k: Optional[torch.Tensor] = None) -> bool:
-    """True when the sm_100a kernels handle this call (Blackwell GPU, bf16/fp16, head_dim 128).
+    """True when the sm_90a kernels handle this call (Hopper GPU, bf16/fp16, head_dim 128).
 
     Other CUDA inputs (e.g. head_dim 64) run the dense torch blocks on the GPU - slow but correct."""
     from ..ops import attn_cuda, cuda_ext
 
-    if not cuda_ext.available_for(q):  # False for anything that is not a Blackwell GPU tensor
+    if not cuda_ext.available_for(q):  # False for anything that is not a Hopper GPU tensor
         return False
     if attn_cuda.is_fp8_kernel_input(q, q if k is None else k):
         return attn_cuda.current_fp8_scales() is not None  # experimental fp8 forward (parallel/api.py)
@@ -413,7 +413,7 @@ def deterministic_mode() -> str:
 
 def cp_backward(plan: CPPlan, dout, q, k, v, out, lse, scale, group, transport="ring",
                 heads_k_stride: int = 1, deterministic: bool = False):
-    # The reference forwards the flag to flash-attn's backward (ring_flash_attn.py:119).  On the sm_100a path out / lse
+    # The reference forwards the flag to flash-attn's backward (ring_flash_attn.py:119).  On the sm_90a path out / lse
     # never depend on timing, dK / dV have one writer per tile and a fixed-order owner-side sum; dQ tiles are added
     # with unordered fp32 L2 reductions.  ``ordered``: launch the key tiles in groups with disjoint query rows
     # (ops/attn_cuda.py:ordered_dq_groups) and, across GPUs, move K/V and dK/dV with the fixed-order ring /

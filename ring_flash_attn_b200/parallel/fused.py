@@ -1,9 +1,9 @@
-"""Fused sm_100a execution of a context-parallel plan.
+"""Fused sm_90a execution of a context-parallel plan.
 
 ``world == 1``: one forward launch and one backward launch over the whole plan.
 ``world > 1`` : the same kernels, with every remote K/V shard arriving through peer-mapped staging
 buffers that the *attention kernel's own communication CTAs* fill over NVLink while the math on the
-local shard runs (``parallel/symm.py`` + ``csrc/comm_sm100.cu``).  No NCCL call is on this path.
+local shard runs (``parallel/symm.py`` + ``csrc/comm_sm90.cu``).  No NCCL call is on this path.
 
 Replaces the per-step Python loops of the reference (flash-attn call + fp32 merge + batch_isend_irecv per ring
 step: /root/reference/ring_flash_attn/ring_flash_attn.py:7-154, zigzag_ring_flash_attn.py:7-199,

@@ -156,7 +156,7 @@ def _out_dtype(q: Tensor) -> torch.dtype:
 
 
 def _fp8_kernel_takes(plan, q: Tensor, k: Tensor, kv_block: int) -> bool:
-    """The fp8 forward kernel (e4m3, head_dim 128, Blackwell GPU) reads one K and one V descale per 128-key tile:
+    """The fp8 forward kernel (e4m3, head_dim 128, Hopper GPU) reads one K and one V descale per 128-key tile:
     descale blocks must be whole tiles (multiples of 128 rows, with every key segment starting on a tile boundary)
     or cover the whole local shard; windows are not instantiated for fp8.  ``RFA_B200_FP8_KERNEL=0`` disables it."""
     import os

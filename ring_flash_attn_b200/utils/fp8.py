@@ -4,7 +4,7 @@ BASELINE.json config 5 asks for stripe attention on block-scaled fp8 Q/K/V.  fp8
 ``descale`` tensor.  e4m3 q / k / v of head size 128 whose descales are per tensor, per head or per token block x head
 (k / v: blocks that are whole 128-key tiles) go straight into the fp8 forward kernel (``kind::f8f6f4``, one byte per
 element on the NVLink wire, scales applied to the fp32 scores / folded into P; ``parallel/api.py:_fp8_kernel_scales``,
-``csrc/attn_fwd_sm100.cu``); everything else (e5m2, scales that vary inside a row such as MX per-32 along head_dim,
+``csrc/attn_fwd_sm90.cu``); everything else (e5m2, scales that vary inside a row such as MX per-32 along head_dim,
 sliding windows, other head sizes) is expanded to bf16 right before the attention call.  The scale layout is
 deliberately general: ``descale.shape[d]`` must divide ``x.shape[d]`` in every dimension, the quotient is the block
 size along that dimension (``float8_e8m0fnu`` scales are accepted as well).  Forward only: fp8 tensors carry no

@@ -1,11 +1,11 @@
-"""`python setup.py build_ext --inplace` (or `python -m ring_flash_attn_b200.build_ext`) builds the sm_100a
+"""`python setup.py build_ext --inplace` (or `python -m ring_flash_attn_b200.build_ext`) builds the sm_90a
 extension next to the sources; `pip install -e .` installs the package in development mode."""
 from setuptools import find_packages, setup
 from setuptools.command.build_ext import build_ext as _build_ext
 
 
 class BuildSm100(_build_ext):
-    def run(self):  # nvcc is driven directly (explicit -gencode arch=compute_100a,code=sm_100a)
+    def run(self):  # nvcc is driven directly (explicit -gencode arch=compute_90a,code=sm_90a)
         from ring_flash_attn_b200 import build_ext
 
         print(build_ext.build(verbose=True))

@@ -1,6 +1,6 @@
 """A torch implementation of the extension's launch entry points, driven by the SAME device work tables.
 
-It lets the CPU suite run the code paths that normally need a B200 - table construction, launch dispatch
+It lets the CPU suite run the code paths that normally need an H100 - table construction, launch dispatch
 (plain / sliding-window / fp8), per-source ring steps, the autograd bridge - end to end against the dense oracle.
 Each function implements the *contract* of its kernel (what the tables mean), not the tile schedule; the tile-level
 index arithmetic is replayed separately in tests/test_tables.py.

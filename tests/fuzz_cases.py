@@ -1,7 +1,7 @@
 """Randomised end-to-end cases for the table-driven launch contract, on CPU.
 
 * ``world1_case(seed)``: the public API at world size 1 through ``tests/fake_ext.py`` (a torch implementation of each
-  launch's contract, driven by the same work tables as the sm_100a kernels) against the dense fp32 oracle: random
+  launch's contract, driven by the same work tables as the sm_90a kernels) against the dense fp32 oracle: random
   shapes, GQA ratios, head sizes, sliding windows, packed documents, causal or not, ordered (deterministic) launch
   groups.
 * ``fused_case(seed)``: the fused multi-GPU launch replayed in one process (``tests/test_fused_emulation.py``) for a

@@ -1,4 +1,4 @@
-"""sm_100a kernels against the plain fp32 PyTorch oracle (run with -m gpu on a B200)."""
+"""sm_90a kernels against the plain fp32 PyTorch oracle (run with -m gpu on an H100)."""
 import math
 
 import pytest
@@ -20,21 +20,7 @@ def _ext():
 def test_extension_is_loaded_and_native():
     C = _ext()
     assert hasattr(C, "attn_fwd") and hasattr(C, "attn_bwd")
-    assert torch.cuda.get_device_capability()[0] == 10, "these tests expect a Blackwell (sm_100) GPU"
-
-
-def test_descriptor_probe_all_forms():
-    import importlib.util
-    import os
-
-    spec = importlib.util.spec_from_file_location(
-        "probe_descriptors", os.path.join(os.path.dirname(__file__), "..", "benchmark", "probe_descriptors.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    C = _ext()
-    for name in mod.MODES:
-        err, mag = mod.run(C, name)
-        assert err < 2e-2 * max(mag, 1.0), f"{name}: max err {err}"
+    assert torch.cuda.get_device_capability()[0] == 9, "these tests expect a Hopper (sm_90) GPU"
 
 
 def _rand(shape, dtype, seed):
@@ -48,7 +34,7 @@ def _rand(shape, dtype, seed):
     (200, 333, 2, 2, 40), (77, 50, 1, 1, None), (300, 300, 2, 2, -1), (512, 1024, 2, 1, None),
 ])
 def test_fwd_block_kernel(dtype, sq, sk, hq, hkv, diag):
-    """One chunk x one segment through the tcgen05 forward kernel vs dense fp32."""
+    """One chunk x one segment through the wgmma forward kernel vs dense fp32."""
     from ring_flash_attn_b200.ops import attn_cuda
 
     q, k, v = _rand((sq, hq, 128), dtype, 1), _rand((sk, hkv, 128), dtype, 2), _rand((sk, hkv, 128), dtype, 3)
@@ -252,22 +238,10 @@ def test_sliding_window_kernels(monkeypatch, fn_name, causal, window):
     assert (kv.grad.float() - rkv.grad).abs().max().item() < 5e-2 * rkv.grad.abs().max().item() + 2e-2
 
 
-def test_fp8_descriptor_probe():
-    """kind::f8f6f4 operand forms of the fp8 forward (benchmark/probe_fp8.py sweeps alternatives on a mismatch)."""
-    C = _ext()
-    g = torch.Generator(device="cuda").manual_seed(0)
-    a = (torch.randn(128, 128, device="cuda", generator=g) * 0.5).to(torch.float8_e4m3fn)
-    b = (torch.randn(128, 128, device="cuda", generator=g) * 0.5).to(torch.float8_e4m3fn)
-    for a_kind, b_kind, ref in ((0, 0, a.float() @ b.float().t()), (1, 1, a.float() @ b.float())):
-        out = C.probe_fp8(a, b, [a_kind, b_kind, 0, -1, -1, -1])
-        torch.cuda.synchronize()
-        assert (out - ref).abs().max().item() < 1e-3 * max(ref.abs().max().item(), 1.0), (a_kind, b_kind)
-
-
 @pytest.mark.parametrize("per_head", [False, True])
 def test_fp8_forward_kernel(monkeypatch, per_head):
-    """Default for per-tensor / per-head descales: e4m3 q/k/v go straight into the forward kernel (kind::f8f6f4 for both GEMMs, P as
-    e4m3 in tensor memory); compared with the oracle on the dequantised tensors at fp8 tolerance."""
+    """Default for per-tensor / per-head descales: e4m3 q/k/v go straight into the forward kernel (e4m3 wgmma for Q K^T, V widened
+    to bf16 in shared memory for P V); compared with the oracle on the dequantised tensors at fp8 tolerance."""
     from ring_flash_attn_b200.ops import cuda_ext
     from ring_flash_attn_b200.utils import fp8
 
@@ -342,7 +316,7 @@ def test_compile_fullgraph_world1(backend):
             pytest.skip(f"inductor toolchain unavailable on this box: {type(e).__name__}")
         raise
     out.backward(dout)
-    assert cuda_ext.launch_counter().value >= before + 6, "compiled function did not reach the sm_100a kernels"
+    assert cuda_ext.launch_counter().value >= before + 6, "compiled function did not reach the sm_90a kernels"
     torch.testing.assert_close(out.float(), ref.float(), atol=1e-2, rtol=1e-2)
     assert (qkv.grad.float() - g_ref.float()).abs().max().item() < 2e-2 * g_ref.float().abs().max().item() + 1e-2
 

@@ -1,4 +1,4 @@
-"""The code paths that normally need a B200 - work tables, launch dispatch (plain / sliding window / fp8), per-source
+"""The code paths that normally need an H100 - work tables, launch dispatch (plain / sliding window / fp8), per-source
 ring steps, autograd bridge - run on CPU against the dense oracle, with the extension replaced by
 ``tests/fake_ext.py`` (a torch implementation of each launch's contract, driven by the same tables)."""
 import os

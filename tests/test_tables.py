@@ -1,4 +1,4 @@
-"""Host-side work tables consumed by the sm_100a kernels (no GPU needed): coverage and exclusivity invariants."""
+"""Host-side work tables consumed by the sm_90a kernels (no GPU needed): coverage and exclusivity invariants."""
 import pytest
 import torch
 
@@ -147,8 +147,9 @@ def _plan_visibility(plan, world):
 
 
 def _replay_forward(items, segs, seg_lo, q_rows, kv_cols):
-    """attn_fwd_sm100.cu: seg_geom / tile_active / tile_needs_mask / tile_needs_lower_mask / the column limits."""
-    T = 128
+    """attn_fwd_sm90.cu: seg_geom / wg_active / wg_needs_mask / wg_needs_lower_mask / the column limits, per 64-row
+    compute warpgroup of a work item."""
+    T, W = 128, 64  # keys per K/V tile, query rows per warpgroup
     vis = torch.zeros(q_rows, kv_cols, dtype=torch.int32)
     for q_row0, n_rows, q_off, seg_begin, seg_count, *_ in items:
         for si in range(seg_begin, seg_begin + seg_count):
@@ -157,17 +158,15 @@ def _replay_forward(items, segs, seg_lo, q_rows, kv_cols):
             last_row = q_off + n_rows - 1
             reach = min(max(last_row + diag + 1, 0), kv_len)
             n_tiles = (reach + T - 1) // T
-            for t in range(2):
-                n_t = min(n_rows, T) if t == 0 else n_rows - T
-                if n_t <= 0:
-                    continue
-                first_row = q_off + t * T
+            for w in range((n_rows + W - 1) // W):
+                n_w = min(n_rows - w * W, W)
+                first_row = q_off + w * W
                 for jj in range(n_tiles):
-                    if not jj * T <= first_row + n_t - 1 + diag:  # tile_active
+                    if not jj * T <= first_row + n_w - 1 + diag:  # wg_active
                         continue
-                    masked = (jj + 1) * T > kv_len or jj * T + T - 1 > first_row + diag
-                    masked = masked or (first_row + T - 1 + lo > jj * T)
-                    for r in range(n_t):
+                    masked = (jj + 1) * T > kv_len or jj * T + T - 1 > first_row + diag  # wg_needs_mask
+                    masked = masked or (first_row + W - 1 + lo > jj * T)  # wg_needs_lower_mask
+                    for r in range(n_w):
                         chunk_row = first_row + r
                         c_lo, c_hi = 0, T - 1
                         if masked:
@@ -175,12 +174,12 @@ def _replay_forward(items, segs, seg_lo, q_rows, kv_cols):
                             c_lo = max(0, min(T, chunk_row + lo - jj * T))
                         if c_hi >= c_lo:
                             a = kv_row0 + jj * T
-                            vis[q_row0 + t * T + r, a + c_lo:a + c_hi + 1] += 1
+                            vis[q_row0 + w * W + r, a + c_lo:a + c_hi + 1] += 1
     return vis
 
 
 def _replay_backward(items, qsegs, q_rows, kv_cols):
-    """attn_bwd_sm100.cu: q_geom, the lse=+inf rows behind q_len, q_lo / q_hi per key."""
+    """attn_bwd_sm90.cu: q_geom, the lse=+inf rows behind q_len, q_lo / q_hi per key."""
     TQ = 64
     vis = torch.zeros(q_rows, kv_cols, dtype=torch.int32)
     owner = torch.zeros(kv_cols, dtype=torch.int32)

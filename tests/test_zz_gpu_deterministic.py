@@ -1,6 +1,4 @@
-"""deterministic=True on the sm_100a path (B200): bitwise reproducible gradients, still equal to the fp32 oracle.
-
-Passed on a B200 at the end of round 2 (profiles/r2/trip_last_deterministic.log).
+"""deterministic=True on the sm_90a path (H100): bitwise reproducible gradients, still equal to the fp32 oracle.
 
 The file name sorts last so that the determinism checks run after every other GPU test file."""
 import pytest
