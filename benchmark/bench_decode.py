@@ -1,0 +1,155 @@
+"""Decode step against a long KV cache: the sm_90a split-KV kernel vs torch SDPA (``enable_gqa=True``) on the same
+local shard, alternating in one run.
+
+One JSON line per (batch, cache length): device-timed microseconds per call, the K + V bytes the call must read, the
+achieved rate and its share of the H100 SXM data-sheet HBM bandwidth (3.35 TB/s; a data-sheet figure, not a measured
+peak), with the card name and power limit.  Under ``torchrun`` (world > 1) every rank holds a shard of that length and
+the line also reports the all-gather + combine time of the cross-rank merge.
+
+    python benchmark/bench_decode.py                      # B in {1, 8}, caches of 32K..512K tokens per rank
+    torchrun --nproc-per-node 2 benchmark/bench_decode.py
+    python benchmark/bench_decode.py --dry-run            # shapes and byte counts only (no GPU)
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from ring_flash_attn_b200.parallel import decode as dec  # noqa: E402
+
+HBM_DATASHEET_BPS = 3.35e12  # H100 SXM data sheet, HBM3
+
+
+def parse_args(argv=None):
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, nargs="+", default=[1, 8])
+    ap.add_argument("--cache", type=int, nargs="+", default=[32768, 131072, 524288], help="tokens per rank")
+    ap.add_argument("--sq", type=int, default=1)
+    ap.add_argument("--hq", type=int, default=32)
+    ap.add_argument("--hkv", type=int, default=8)
+    ap.add_argument("--head-dim", type=int, default=128)
+    ap.add_argument("--iters", type=int, default=50)
+    ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--sm-count", type=int, default=132, help="used by --dry-run only")
+    ap.add_argument("--dry-run", action="store_true")
+    return ap.parse_args(argv)
+
+
+def shapes(args, sm_count):
+    """One dict per configuration: shapes, split count and the K + V bytes one call reads (bf16)."""
+    for b in args.batch:
+        for s in args.cache:
+            yield dict(batch=b, cache_tokens=s, sq=args.sq, hq=args.hq, hkv=args.hkv, head_dim=args.head_dim,
+                       splits=dec.num_splits(b, args.sq, args.hq, args.hkv, s, sm_count),
+                       kv_bytes=b * s * args.hkv * args.head_dim * 2 * 2)
+
+
+def card():
+    name = torch.cuda.get_device_name(0)
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
+                            str(torch.cuda.current_device())], stdout=subprocess.PIPE, text=True, timeout=30)
+        power = r.stdout.strip() or "unknown"
+    except (OSError, subprocess.SubprocessError):
+        power = "unknown"
+    return name, power
+
+
+def time_us(fn, iters, warmup):
+    for _ in range(warmup):
+        fn()
+    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    start.record()
+    for _ in range(iters):
+        fn()
+    end.record()
+    end.synchronize()
+    return start.elapsed_time(end) * 1e3 / iters
+
+
+def main():
+    args = parse_args()
+    if args.dry_run:
+        for cfg in shapes(args, args.sm_count):
+            print(json.dumps(cfg))
+        return
+    import torch.distributed as dist
+    import torch.nn.functional as F
+
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_decode.py needs a CUDA device (use --dry-run without one)")
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    if world > 1:
+        torch.cuda.set_device(int(os.environ["LOCAL_RANK"]))
+        dist.init_process_group("nccl")
+    rank = dist.get_rank() if world > 1 else 0
+    dev = torch.device("cuda", torch.cuda.current_device())
+    name, power = card()
+    sm = torch.cuda.get_device_properties(dev).multi_processor_count
+    for cfg in shapes(args, sm):
+        b, s, d = cfg["batch"], cfg["cache_tokens"], args.head_dim
+        torch.manual_seed(rank)
+        q = torch.randn(b, args.sq, args.hq, d, device=dev, dtype=torch.bfloat16)
+        kc = torch.randn(b, s, args.hkv, d, device=dev, dtype=torch.bfloat16)
+        vc = torch.randn(b, s, args.hkv, d, device=dev, dtype=torch.bfloat16)
+        sl = torch.full((b,), s, dtype=torch.int32, device=dev)
+        scale = d ** -0.5
+
+        def ours():
+            dec.kernel_decode(q, kc, vc, sl, None, None, True, scale)
+
+        # SDPA reads the same shard through (B, H, S, D) views
+        qt, kt, vt = q.transpose(1, 2), kc.transpose(1, 2), vc.transpose(1, 2)
+
+        def sdpa():
+            F.scaled_dot_product_attention(qt, kt, vt, scale=scale, enable_gqa=True)
+
+        rows = {"ours": [], "sdpa": []}
+        sdpa_err = None
+        for _ in range(3):  # alternate the two in one run
+            rows["ours"].append(time_us(ours, args.iters, args.warmup))
+            if sdpa_err is None:
+                try:
+                    rows["sdpa"].append(time_us(sdpa, args.iters, args.warmup))
+                except RuntimeError as e:  # e.g. out of memory when SDPA expands the kv heads
+                    sdpa_err = str(e).splitlines()[0][:200]
+                    torch.cuda.empty_cache()
+        res = dict(cfg, dtype="bf16", world=world, card=name, power_limit=power)
+        for k, ts in rows.items():
+            if ts:
+                us = min(ts)
+                res[f"{k}_us"] = round(us, 2)
+                res[f"{k}_us_all"] = [round(t, 2) for t in ts]
+                res[f"{k}_GBps"] = round(cfg["kv_bytes"] / (us * 1e-6) / 1e9, 1)
+                res[f"{k}_share_of_datasheet_hbm"] = round(cfg["kv_bytes"] / (us * 1e-6) / HBM_DATASHEET_BPS, 3)
+        if sdpa_err:
+            res["sdpa_error"] = sdpa_err
+        if world > 1:
+            C = dec.cuda_ext.load()
+            n_out = b * args.sq * args.hq * d
+            mine = torch.randn(n_out + b * args.hq * args.sq, device=dev)
+            out = torch.empty(q.shape, dtype=q.dtype, device=dev)
+            lse = torch.empty(b, args.hq, args.sq, device=dev)
+
+            def merge():
+                C.decode_combine(dec._gather(mine, None, world), out, lse)
+
+            res["allgather_combine_us"] = round(time_us(merge, args.iters, args.warmup), 2)
+            res["full_call_us"] = round(time_us(
+                lambda: dec.kernel_decode(q, kc, vc, sl, None, None, True, scale, None, world), args.iters,
+                args.warmup), 2)
+        if rank == 0:
+            print(json.dumps(res), flush=True)
+        del q, kc, vc
+        torch.cuda.empty_cache()
+    if world > 1:
+        dist.destroy_process_group()
+
+
+if __name__ == "__main__":
+    main()

@@ -6,6 +6,7 @@ The Hugging Face adapter is imported lazily so that ``import ring_flash_attn_b20
 """
 from .parallel.api import *  # noqa: F401,F403
 from .parallel.api import __all__ as _api_all
+from .parallel.decode import cp_flash_attn_with_kvcache
 
 __version__ = "0.2.0"
 
@@ -25,4 +26,4 @@ def __getattr__(name):
     raise AttributeError(f"module {__name__!r} has no attribute {name!r}")
 
 
-__all__ = list(_api_all) + list(_LAZY)
+__all__ = list(_api_all) + ["cp_flash_attn_with_kvcache"] + list(_LAZY)

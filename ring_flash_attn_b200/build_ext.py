@@ -20,7 +20,8 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-DRFA_BUILD"]
 if os.environ.get("RFA_TRACE", "0") == "1":
     NVCC_FLAGS.append("-DRFA_TRACE")
-CU_SOURCES = ["attn_fwd_sm90.cu", "attn_bwd_sm90.cu", "tensor_map.cu", "lse_layout.cu", "comm_sm90.cu"]
+CU_SOURCES = ["attn_fwd_sm90.cu", "attn_bwd_sm90.cu", "tensor_map.cu", "lse_layout.cu", "comm_sm90.cu",
+              "decode_sm90.cu"]
 CPP_SOURCES = ["bindings.cpp", "peer_mem.cpp"]
 
 

@@ -6,6 +6,7 @@
 #include <cstdlib>
 
 #include "attn_common.h"
+#include "decode.h"
 #include "peer_mem.h"
 
 namespace {
@@ -396,6 +397,84 @@ at::Tensor lse_unflatten(const at::Tensor& lse, const at::Tensor& cu, int64_t ma
   return out;
 }
 
+// Split-KV decode (csrc/decode_sm90.cu).  q (B, Sq, Hq, D); k_cache / v_cache (B, S_cap, Hkv, D) with mergeable
+// batch and sequence dimensions; seqlens (B,) int32; k_new / v_new (B, Sq, Hkv, D) contiguous, appended to the caches
+// before attention when given.  part: fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq), see DecodeParams.
+void decode_fwd(const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
+                const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
+                double scale, at::Tensor& part) {
+  const c10::cuda::CUDAGuard guard(q.device());
+  TORCH_CHECK(q.dim() == 4 && k_cache.dim() == 4 && v_cache.dim() == 4, "decode_fwd: 4-D q / k_cache / v_cache");
+  TORCH_CHECK(k_cache.sizes() == v_cache.sizes(), "decode_fwd: k_cache and v_cache shapes differ");
+  TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(),
+              "decode_fwd: caches must have q's dtype");
+  const int64_t B = q.size(0), sq = q.size(1), hq = q.size(2), d = q.size(3);
+  const int64_t s_cap = k_cache.size(1), hkv = k_cache.size(2);
+  TORCH_CHECK(k_cache.size(0) == B && k_cache.size(3) == d, "decode_fwd: cache shape does not match q");
+  TORCH_CHECK(q.stride(3) == 1 && q.stride(0) == sq * q.stride(1), "decode_fwd: q must be (B, Sq) mergeable");
+  TORCH_CHECK((q.stride(1) * 2) % 16 == 0 && (q.stride(2) * 2) % 16 == 0 &&
+                  reinterpret_cast<uintptr_t>(q.data_ptr()) % 16 == 0,
+              "decode_fwd: q rows must be 16-byte aligned");
+  for (const at::Tensor* c : {&k_cache, &v_cache})
+    TORCH_CHECK(c->stride(3) == 1 && c->stride(0) == s_cap * c->stride(1),
+                "decode_fwd: the cache's batch and sequence dimensions must be mergeable (stride(0) == S_cap * stride(1))");
+  TORCH_CHECK(seqlens.scalar_type() == at::kInt && seqlens.is_cuda() && seqlens.is_contiguous() && seqlens.numel() == B,
+              "decode_fwd: cache_seqlens must be (B,) int32 on the device");
+  TORCH_CHECK(part.scalar_type() == at::kFloat && part.is_contiguous() && part.dim() == 2 && part.size(0) >= 1 &&
+                  part.size(1) == B * sq * hq * d + B * hq * sq,
+              "decode_fwd: part must be fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq)");
+  TORCH_CHECK(k_new.has_value() == v_new.has_value(), "decode_fwd: pass both k_new and v_new or neither");
+  const void* kn = nullptr;
+  const void* vn = nullptr;
+  if (k_new.has_value()) {
+    for (const at::Tensor* t : {&*k_new, &*v_new})
+      TORCH_CHECK(t->is_contiguous() && t->scalar_type() == q.scalar_type() && t->dim() == 4 && t->size(0) == B &&
+                      t->size(1) == sq && t->size(2) == hkv && t->size(3) == d,
+                  "decode_fwd: k_new / v_new must be contiguous (B, Sq, Hkv, D) in q's dtype");
+    kn = k_new->data_ptr();
+    vn = v_new->data_ptr();
+  }
+  const int64_t n_splits = part.size(0);
+  const int64_t tiles = (s_cap + 127) / 128;
+  rfa::DecodeParams p{};
+  p.q = q.data_ptr();
+  p.q_row_stride = q.stride(1);
+  p.q_head_stride = q.stride(2);
+  p.seqlens = seqlens.data_ptr<int>();
+  p.part = part.data_ptr<float>();
+  p.part_stride = part.size(1);
+  p.batch = static_cast<int>(B);
+  p.sq = static_cast<int>(sq);
+  p.hq = static_cast<int>(hq);
+  p.hkv = static_cast<int>(hkv);
+  p.s_cap = static_cast<int>(s_cap);
+  p.tiles_per_split = static_cast<int>((tiles + n_splits - 1) / n_splits);
+  p.n_new = kn != nullptr ? static_cast<int>(sq) : 0;
+  p.causal = causal ? 1 : 0;
+  p.scale_log2 = static_cast<float>(scale * 1.4426950408889634);
+  const TensorView kv{k_cache.data_ptr(), B * s_cap, static_cast<int>(hkv), k_cache.stride(1), k_cache.stride(2)};
+  const TensorView vv{v_cache.data_ptr(), B * s_cap, static_cast<int>(hkv), v_cache.stride(1), v_cache.stride(2)};
+  check(rfa::decode_fwd_launch(dtype_code(q), kv, vv, kn, vn, p, static_cast<int>(n_splits), static_cast<int>(d),
+                               at::cuda::getCurrentCUDAStream()));
+}
+
+// Merges the partials of decode_fwd (or gathered per-rank partials, same layout): out (B, Sq, Hq, D) contiguous in
+// bf16 / fp16 / fp32, lse (B, Hq, Sq) fp32 contiguous.
+void decode_combine(const at::Tensor& parts, at::Tensor& out, at::Tensor& lse) {
+  const c10::cuda::CUDAGuard guard(parts.device());
+  TORCH_CHECK(out.dim() == 4 && out.is_contiguous() && out.is_cuda(), "decode_combine: out must be contiguous (B, Sq, Hq, D)");
+  const int64_t B = out.size(0), sq = out.size(1), hq = out.size(2), d = out.size(3);
+  TORCH_CHECK(parts.scalar_type() == at::kFloat && parts.is_contiguous() && parts.dim() == 2 && parts.size(0) >= 1 &&
+                  parts.size(1) == B * sq * hq * d + B * hq * sq,
+              "decode_combine: parts must be fp32 (P, B*Sq*Hq*D + B*Hq*Sq)");
+  TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == B * hq * sq,
+              "decode_combine: lse must be fp32 (B, Hq, Sq)");
+  const int out_dtype = out.scalar_type() == at::kFloat ? -1 : dtype_code(out);
+  check(rfa::decode_combine_launch(parts.data_ptr<float>(), parts.size(1), static_cast<int>(parts.size(0)),
+                                   static_cast<int>(B), static_cast<int>(sq), static_cast<int>(hq), static_cast<int>(d),
+                                   out.data_ptr(), out_dtype, lse.data_ptr<float>(), at::cuda::getCurrentCUDAStream()));
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -443,5 +522,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attn_bwd", &attn_bwd);
   m.def("lse_flatten", &lse_flatten);
   m.def("lse_unflatten", &lse_unflatten);
+  m.def("decode_fwd", &decode_fwd);
+  m.def("decode_combine", &decode_combine);
   rfa::bind_peer_mem(m);
 }

@@ -1,0 +1,38 @@
+// Host/device structures of the split-KV decode kernels (csrc/decode_sm90.cu).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "attn_common.h"
+
+namespace rfa {
+
+// Partial results live in one fp32 buffer per split (or per rank): the (b, t, h) rows of `out` (rows x head_dim),
+// followed by `lse` in the (b, h, t) order of the public softmax_lse.  part_stride = elements per split.
+struct DecodeParams {
+  const void* q;           // (B * Sq, Hq, D) view of (B, Sq, Hq, D)
+  long long q_row_stride;  // elements between consecutive (b, t)
+  long long q_head_stride;
+  const int* seqlens;      // (B,) valid cached rows of this rank's shard
+  float* part;             // (n_splits, part_stride)
+  long long part_stride;
+  int batch, sq, hq, hkv;
+  int s_cap;               // cache rows per sequence
+  int tiles_per_split;     // 128-key tiles of one sequence handled by one split
+  int n_new;               // keys appended to this shard by this call (0 on every rank but the append rank)
+  int causal;              // appended key u is visible to query token t only if u <= t
+  float scale_log2;        // softmax scale * log2(e)
+};
+
+// Appends k_new / v_new (B, Sq, Hkv, D), contiguous, at rows [seqlens[b], seqlens[b] + Sq) of the caches (rows past
+// the capacity are dropped), then runs the split-KV kernel.  k_new == nullptr: attention only.
+const char* decode_fwd_launch(int dtype, const TensorView& k_cache, const TensorView& v_cache, const void* k_new,
+                              const void* v_new, const DecodeParams& p, int n_splits, int head_dim,
+                              cudaStream_t stream);
+
+// Merges n_parts partials (part_stride elements apart) row by row in partial order.  out_dtype: kDtypeBF16,
+// kDtypeFP16, or -1 for fp32.
+const char* decode_combine_launch(const float* parts, long long part_stride, int n_parts, int batch, int sq, int hq,
+                                  int head_dim, void* out, int out_dtype, float* lse, cudaStream_t stream);
+
+}  // namespace rfa

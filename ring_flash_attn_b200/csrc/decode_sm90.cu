@@ -1,0 +1,402 @@
+// Split-KV ("flash-decoding") attention for sm_90a: a few new query tokens against a long K/V cache.
+//
+// One CTA = (split of the key range) x (64-row tile of packed query rows) x (sequence, kv head).  The query rows of
+// one kv head are packed into the wgmma M dimension as (token t, head-in-group g) -> row t * G + g, so that a GQA
+// group reads each K/V tile once instead of once per query head.  The CTA streams the 128-key tiles of its split
+// with TMA through an mbarrier ring and runs the forward kernel's online softmax; it writes a normalised fp32
+// partial out and its lse.  decode_combine_kernel merges partials (over the splits of one rank, and again over the
+// gathered partials of all ranks): lse = logsumexp(lse_p), out = sum_p exp(lse_p - lse) out_p, in partial order.
+//
+// Roles (160 threads): warpgroup 0 computes (S = Q K^T, mask, softmax, O += P V, epilogue); warp 4 is the TMA
+// producer (one thread).
+//
+// Visibility: key j of the shard is visible to query token t iff j < seqlens[b] + n_vis(t), where n_vis(t) counts
+// the keys this call appended to this shard that t may see (0 on every rank but the append rank; t + 1 when causal,
+// Sq otherwise).  Cache rows at or past that limit are never read into a result: their K columns are masked to
+// -inf and their V rows are zeroed in shared memory before P V (the cache may hold anything there, NaN included).
+#include <math_constants.h>
+
+#include <type_traits>
+
+#include "decode.h"
+#include "sm90_ptx.cuh"
+
+namespace rfa {
+
+namespace dec {
+
+constexpr int kTile = 128;    // keys per K / V tile
+constexpr int kRows = 64;     // packed query rows per CTA (one wgmma M)
+constexpr int kStages = 6;    // K/V ring slots (one key tile takes two: K, then V)
+constexpr int kThreads = 160;  // one compute warpgroup + one producer warp
+constexpr int kKHalfBytes = kTile * 128;  // one 64-element-wide (128-byte) swizzled K / V sub-tile
+constexpr int kQHalfBytes = kRows * 128;  // the same for the query tile
+
+template <int kD>
+constexpr int smem_bytes() {
+  return kRows * kD * 2 + kStages * kTile * kD * 2 + 1024 /*barriers*/ + 1024 /*align slack*/;
+}
+
+struct Barriers {
+  uint64_t kv_full[kStages];
+  uint64_t kv_empty[kStages];
+};
+
+// Keys of the shard visible to token t (see the file comment), at most the capacity.
+__device__ __forceinline__ int key_limit(const DecodeParams& p, int seqlen, int t) {
+  const int n_vis = p.n_new == 0 ? 0 : (p.causal ? t + 1 : p.sq);
+  const int lim = seqlen + n_vis;
+  return lim < p.s_cap ? lim : p.s_cap;
+}
+
+template <typename T, int kD>
+__global__ void __launch_bounds__(kThreads, 1)
+decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
+              const __grid_constant__ DecodeParams p) {
+  static_assert(kD == 64 || kD == 128, "head dim 64 or 128");
+  constexpr int kSubTiles = kD / 64;
+  constexpr int kSlotBytes = kTile * kD * 2;
+  constexpr uint32_t kTxBytes = kSlotBytes;
+  const int split = blockIdx.x;
+  const int b = blockIdx.z / p.hkv, kv_head = blockIdx.z % p.hkv;
+  const int group = p.hq / p.hkv;
+  const int n_rows = p.sq * group;  // packed query rows of this kv head
+  const int row0 = blockIdx.y * kRows;
+  const int rows_here = n_rows - row0 < kRows ? n_rows - row0 : kRows;
+  int seqlen = p.seqlens[b];
+  seqlen = seqlen < 0 ? 0 : (seqlen > p.s_cap ? p.s_cap : seqlen);
+  // the last row of the tile sees the most keys (the limit never decreases with t)
+  const int kmax = key_limit(p, seqlen, (row0 + rows_here - 1) / group);
+  const int j0 = split * p.tiles_per_split;
+  int j1 = (kmax + kTile - 1) / kTile;
+  if (j1 > j0 + p.tiles_per_split) j1 = j0 + p.tiles_per_split;
+  const int n_tiles = j1 - j0;  // <= 0: this split starts past the visible keys
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem_q = smem;
+  uint8_t* smem_kv = smem + kRows * kD * 2;
+  Barriers* bars = reinterpret_cast<Barriers*>(smem_kv + kStages * kSlotBytes);
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tm_k);
+    tma_prefetch_desc(&tm_v);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&bars->kv_full[i], 1);
+      mbar_init(&bars->kv_empty[i], 4);  // one arrival per compute warp
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (threadIdx.x >= 128) {
+    // ------------------------------------------------------------------ TMA producer
+    if (threadIdx.x == 128) {
+      uint32_t slot = 0, phase = 0;
+      for (int jj = 0; jj < n_tiles; ++jj) {
+        const int row = b * p.s_cap + (j0 + jj) * kTile;  // rows past the tensor's end arrive as zeros
+        for (int kv = 0; kv < 2; ++kv) {
+          mbar_wait(&bars->kv_empty[slot], phase ^ 1);
+          uint8_t* dst = smem_kv + slot * kSlotBytes;
+          mbar_arrive_expect_tx(&bars->kv_full[slot], kTxBytes);
+#pragma unroll
+          for (int h = 0; h < kSubTiles; ++h)
+            tma_load_3d(dst + h * kKHalfBytes, kv == 0 ? &tm_k : &tm_v, &bars->kv_full[slot], 64 * h, kv_head, row);
+          if (++slot == kStages) {
+            slot = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- compute warpgroup
+  const int tid = threadIdx.x;
+  const int lane = tid & 31;
+  const bool warp_leader = lane == 0;
+  const int r_base = 16 * (tid >> 5) + (lane >> 2);  // this thread's rows: r_base, r_base + 8
+  const int quad_col = 2 * (lane & 3);                // its columns: 8 j + quad_col + {0, 1}
+  const T* q = reinterpret_cast<const T*>(p.q);
+
+  // Q tile: packed rows in the 128-byte swizzled K-major layout TMA would write; rows past the group are zero
+  constexpr int kChunks = kD / 8;  // 16-byte chunks per row
+#pragma unroll 4
+  for (int idx = tid; idx < kRows * kChunks; idx += 128) {
+    const int r = idx / kChunks, c = idx % kChunks;
+    uint4 val = make_uint4(0u, 0u, 0u, 0u);
+    if (r < rows_here) {
+      const int pr = row0 + r;
+      const int t = pr / group, head = kv_head * group + pr % group;
+      val = *reinterpret_cast<const uint4*>(q + (static_cast<long long>(b) * p.sq + t) * p.q_row_stride +
+                                            head * p.q_head_stride + 8 * c);
+    }
+    *reinterpret_cast<uint4*>(smem_q + (c >> 3) * kQHalfBytes + r * 128 + (((c & 7) ^ (r & 7)) << 4)) = val;
+  }
+  fence_proxy_async_smem();
+  named_bar_sync(1, 128);
+
+  int lim[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r_base + 8 * h;
+    lim[h] = r < rows_here ? key_limit(p, seqlen, (row0 + r) / group) : 0;
+  }
+  float o[kD / 2];
+#pragma unroll
+  for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
+  float m2[2] = {-CUDART_INF_F, -CUDART_INF_F};
+  float l[2] = {0.f, 0.f};
+  const float t2 = p.scale_log2;
+
+  const uint64_t q_desc = gmma_desc(smem_u32(smem_q), 0);         // K-major A
+  const uint64_t k_desc0 = gmma_desc(smem_u32(smem_kv), 0);       // K tile, K-major B
+  const uint64_t v_desc0 = gmma_desc(smem_u32(smem_kv), kKHalfBytes);  // V tile, MN-major B
+
+  uint32_t slot = 0, phase = 0;
+  for (int jj = 0; jj < n_tiles; ++jj) {
+    const uint32_t k_slot = slot, k_phase = phase;
+    if (++slot == kStages) {
+      slot = 0;
+      phase ^= 1;
+    }
+    const uint32_t v_slot = slot, v_phase = phase;
+    if (++slot == kStages) {
+      slot = 0;
+      phase ^= 1;
+    }
+    const int key0 = (j0 + jj) * kTile;
+
+    // ---- S = Q K^T
+    mbar_wait(&bars->kv_full[k_slot], k_phase);
+    float s[64];
+    const uint64_t k_desc = gmma_desc_add(k_desc0, k_slot * kSlotBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kD / 16; ++k)
+      Gmma<T>::template ss128<0, 0>(s, gmma_desc_add(q_desc, (k >> 2) * kQHalfBytes + (k & 3) * 32),
+                                    gmma_desc_add(k_desc, (k >> 2) * kKHalfBytes + (k & 3) * 32), k > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    __syncwarp();
+    if (warp_leader) mbar_arrive(&bars->kv_empty[k_slot]);
+
+    // ---- mask keys at or past each row's limit
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (key0 + kTile > lim[h]) {
+        const int c_lim = lim[h] - key0;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            if (8 * j + quad_col + e >= c_lim) s[4 * j + 2 * h + e] = -CUDART_INF_F;
+          }
+        }
+      }
+    }
+
+    // ---- online softmax (two rows per thread; a row lives in the 4 threads of a quad)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -CUDART_INF_F;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) mx = fmaxf(mx, fmaxf(s[4 * j + 2 * h], s[4 * j + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m2[h], mx * t2);
+      const float f = m_new == -CUDART_INF_F ? 1.f : fast_exp2(m2[h] - m_new);
+      m2[h] = m_new;
+      l[h] *= f;
+#pragma unroll
+      for (int j = 0; j < kD / 8; ++j) {
+        o[4 * j + 2 * h] *= f;
+        o[4 * j + 2 * h + 1] *= f;
+      }
+      const float mc = m_new == -CUDART_INF_F ? 0.f : m_new;
+      float sum = 0.f;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float x = fast_exp2(fmaf(s[4 * j + 2 * h + e], t2, -mc));
+          s[4 * j + 2 * h + e] = x;
+          sum += x;
+        }
+      }
+      l[h] += sum;
+    }
+    uint32_t pa[kTile / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < kTile / 16; ++kk) pack_a<T>(pa[kk], s, kk);
+
+    // ---- O += P V
+    mbar_wait(&bars->kv_full[v_slot], v_phase);
+    uint8_t* v_tile = smem_kv + v_slot * kSlotBytes;
+    if (key0 + kTile > kmax) {
+      // V rows no query row may see: zero them (P is 0 there, but 0 * NaN is not)
+      const int z0 = kmax - key0;
+      for (int idx = tid; idx < kSubTiles * (kTile - z0) * 8; idx += 128) {
+        const int h = idx / ((kTile - z0) * 8), rem = idx % ((kTile - z0) * 8);
+        *reinterpret_cast<uint4*>(v_tile + h * kKHalfBytes + (z0 + rem / 8) * 128 + (rem % 8) * 16) =
+            make_uint4(0u, 0u, 0u, 0u);
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1, 128);
+    }
+    const uint64_t v_desc = gmma_desc_add(v_desc0, v_slot * kSlotBytes);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kTile / 16; ++kk) gmma_rs<T, kD>(o, pa[kk], gmma_desc_add(v_desc, kk * 2048), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(o);
+    __syncwarp();
+    if (warp_leader) mbar_arrive(&bars->kv_empty[v_slot]);
+  }
+
+  // ------------------------------------------------------------------ epilogue: O / l -> partial out, lse
+  const long long n_out = static_cast<long long>(p.batch) * p.sq * p.hq;  // rows of out
+  float* part = p.part + split * p.part_stride;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float lt = l[h];
+    lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+    lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+    const int r = r_base + 8 * h;
+    if (r >= rows_here) continue;
+    const int pr = row0 + r;
+    const int t = pr / group, head = kv_head * group + pr % group;
+    const float inv = lt > 0.f ? 1.0f / lt : 0.f;
+    float* out_row = part + ((static_cast<long long>(b) * p.sq + t) * p.hq + head) * kD;
+#pragma unroll
+    for (int j = 0; j < kD / 8; ++j)
+      *reinterpret_cast<float2*>(out_row + 8 * j + quad_col) =
+          make_float2(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
+    if ((lane & 3) == 0) {
+      const float lse = lt > 0.f ? (m2[h] + __log2f(lt)) * 0.6931471805599453f : -CUDART_INF_F;
+      part[n_out * kD + (static_cast<long long>(b) * p.hq + head) * p.sq + t] = lse;
+    }
+  }
+}
+
+// One block per (b, t) row of the new keys, blockIdx.y selects K or V.  16-byte chunks; rows past the capacity
+// are dropped.
+__global__ void decode_append_kernel(uint8_t* k_cache, uint8_t* v_cache, long long row_stride_bytes,
+                                     long long head_stride_bytes, const uint8_t* k_new, const uint8_t* v_new,
+                                     const int* seqlens, int sq, int hkv, int row_bytes, int s_cap) {
+  const int b = blockIdx.x / sq, t = blockIdx.x % sq;
+  const int row = seqlens[b] + t;
+  if (row < 0 || row >= s_cap) return;
+  uint8_t* dst = (blockIdx.y == 0 ? k_cache : v_cache) + (static_cast<long long>(b) * s_cap + row) * row_stride_bytes;
+  const uint8_t* src = (blockIdx.y == 0 ? k_new : v_new) + static_cast<long long>(blockIdx.x) * hkv * row_bytes;
+  const int chunks = row_bytes / 16;
+  for (int idx = threadIdx.x; idx < hkv * chunks; idx += blockDim.x) {
+    const int head = idx / chunks, c = idx % chunks;
+    *reinterpret_cast<uint4*>(dst + head * head_stride_bytes + 16 * c) =
+        *reinterpret_cast<const uint4*>(src + static_cast<long long>(head) * row_bytes + 16 * c);
+  }
+}
+
+template <typename OutT>
+__device__ __forceinline__ void store_out(OutT* p, float x) {
+  if constexpr (std::is_same_v<OutT, float>) *p = x;
+  else if constexpr (std::is_same_v<OutT, __nv_bfloat16>) *p = __float2bfloat16_rn(x);
+  else *p = __float2half_rn(x);
+}
+
+// One warp per (b, t, h) row.  Partials with lse = -inf (no visible key) are skipped, so their out is never read.
+template <typename OutT>
+__global__ void decode_combine_kernel(const float* parts, long long part_stride, int n_parts, int sq, int hq,
+                                      int head_dim, long long n_rows, OutT* out, float* lse_out) {
+  const long long n = static_cast<long long>(blockIdx.x) * (blockDim.x / 32) + threadIdx.x / 32;
+  if (n >= n_rows) return;
+  const int lane = threadIdx.x & 31;
+  const long long b = n / (static_cast<long long>(sq) * hq);
+  const int t = static_cast<int>((n / hq) % sq), h = static_cast<int>(n % hq);
+  const long long li = (b * hq + h) * sq + t;
+  const float* lse_in = parts + n_rows * head_dim + li;
+  float mx = -CUDART_INF_F;
+  for (int i = 0; i < n_parts; ++i) mx = fmaxf(mx, lse_in[i * part_stride]);
+  float lse = -CUDART_INF_F;
+  if (mx != -CUDART_INF_F) {
+    float sum = 0.f;
+    for (int i = 0; i < n_parts; ++i) {
+      const float x = lse_in[i * part_stride];
+      if (x != -CUDART_INF_F) sum += expf(x - mx);
+    }
+    lse = mx + logf(sum);
+  }
+  for (int d = lane; d < head_dim; d += 32) {
+    float acc = 0.f;
+    if (lse != -CUDART_INF_F) {
+      for (int i = 0; i < n_parts; ++i) {
+        const float x = lse_in[i * part_stride];
+        if (x != -CUDART_INF_F) acc += expf(x - lse) * parts[i * part_stride + n * head_dim + d];
+      }
+    }
+    store_out(out + n * head_dim + d, acc);
+  }
+  if (lane == 0) lse_out[li] = lse;
+}
+
+}  // namespace dec
+
+const char* decode_fwd_launch(int dtype, const TensorView& k_cache, const TensorView& v_cache, const void* k_new,
+                              const void* v_new, const DecodeParams& p, int n_splits, int head_dim,
+                              cudaStream_t stream) {
+  if (head_dim != 64 && head_dim != 128) return "the sm_90a decode kernel is instantiated for head_dim 64 and 128";
+  if (dtype != kDtypeBF16 && dtype != kDtypeFP16) return "the sm_90a decode kernel takes bf16 / fp16";
+  if (p.hkv <= 0 || p.hq % p.hkv != 0) return "query heads must be a multiple of kv heads";
+  if (k_cache.row_stride != v_cache.row_stride || k_cache.head_stride != v_cache.head_stride)
+    return "k_cache and v_cache must have the same strides";
+  CUtensorMap tk, tv;
+  if (const char* e = make_tensor_map(&tk, k_cache, 2, dec::kTile, head_dim)) return e;
+  if (const char* e = make_tensor_map(&tv, v_cache, 2, dec::kTile, head_dim)) return e;
+  if (k_new != nullptr && p.n_new > 0) {
+    dec::decode_append_kernel<<<dim3(p.batch * p.sq, 2), 128, 0, stream>>>(
+        static_cast<uint8_t*>(k_cache.ptr), static_cast<uint8_t*>(v_cache.ptr), k_cache.row_stride * 2,
+        k_cache.head_stride * 2, static_cast<const uint8_t*>(k_new), static_cast<const uint8_t*>(v_new), p.seqlens,
+        p.sq, p.hkv, head_dim * 2, p.s_cap);
+  }
+  const int row_tiles = (p.sq * (p.hq / p.hkv) + dec::kRows - 1) / dec::kRows;
+  dim3 grid(n_splits, row_tiles, p.batch * p.hkv), block(dec::kThreads, 1, 1);
+  cudaError_t err = cudaSuccess;
+  auto launch = [&](auto kern, int smem) {
+    err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (err == cudaSuccess) kern<<<grid, block, smem, stream>>>(tk, tv, p);
+  };
+  if (dtype == kDtypeBF16) {
+    if (head_dim == 128) launch(dec::decode_kernel<__nv_bfloat16, 128>, dec::smem_bytes<128>());
+    else launch(dec::decode_kernel<__nv_bfloat16, 64>, dec::smem_bytes<64>());
+  } else {
+    if (head_dim == 128) launch(dec::decode_kernel<__half, 128>, dec::smem_bytes<128>());
+    else launch(dec::decode_kernel<__half, 64>, dec::smem_bytes<64>());
+  }
+  if (err != cudaSuccess) return cudaGetErrorString(err);
+  err = cudaGetLastError();
+  return err == cudaSuccess ? nullptr : cudaGetErrorString(err);
+}
+
+const char* decode_combine_launch(const float* parts, long long part_stride, int n_parts, int batch, int sq, int hq,
+                                  int head_dim, void* out, int out_dtype, float* lse, cudaStream_t stream) {
+  const long long n_rows = static_cast<long long>(batch) * sq * hq;
+  if (n_rows == 0) return nullptr;
+  constexpr int kWarps = 8;
+  const unsigned blocks = static_cast<unsigned>((n_rows + kWarps - 1) / kWarps);
+  if (out_dtype == kDtypeBF16)
+    dec::decode_combine_kernel<<<blocks, 32 * kWarps, 0, stream>>>(parts, part_stride, n_parts, sq, hq, head_dim,
+                                                                   n_rows, static_cast<__nv_bfloat16*>(out), lse);
+  else if (out_dtype == kDtypeFP16)
+    dec::decode_combine_kernel<<<blocks, 32 * kWarps, 0, stream>>>(parts, part_stride, n_parts, sq, hq, head_dim,
+                                                                   n_rows, static_cast<__half*>(out), lse);
+  else
+    dec::decode_combine_kernel<<<blocks, 32 * kWarps, 0, stream>>>(parts, part_stride, n_parts, sq, hq, head_dim,
+                                                                   n_rows, static_cast<float*>(out), lse);
+  const cudaError_t err = cudaGetLastError();
+  return err == cudaSuccess ? nullptr : cudaGetErrorString(err);
+}
+
+}  // namespace rfa

@@ -1,0 +1,234 @@
+"""Context-parallel decoding over a sharded KV cache: ``cp_flash_attn_with_kvcache``.
+
+After a prefill with any scheme, rank ``r`` holds its shard of K and V.  Without windows or positional biases,
+decode attention does not depend on where a cached key sits, so every rank attends the new query tokens to its own
+shard, and the per-rank partial ``(out, lse)`` results are merged with the online-softmax identity
+``lse = logsumexp_r(lse_r)``, ``out = sum_r exp(lse_r - lse) out_r``.  The only traffic between ranks is one
+all-gather of those partials (a few KB per layer).
+
+On Hopper the local step is the split-KV kernel of ``csrc/decode_sm90.cu``: the query heads of a GQA group and the
+new tokens share the wgmma M dimension, one sequence's keys are spread over many CTAs, and one combine kernel merges
+the per-split partials and then, with the same code, the gathered per-rank partials.  Every rank combines the same
+gathered partials in rank order, so ``out`` and ``lse`` are bitwise identical on every rank.
+
+The dense path (CPU / gloo, other GPUs, ``RFA_B200_FORCE_TORCH=1``, and shapes the kernel is not instantiated for)
+computes the local partial with ``ops.dense.block_fwd`` and merges the gathered partials with
+``ops.merge.merge_partial`` in the same rank order.
+"""
+from __future__ import annotations
+
+import functools
+import warnings
+from typing import Optional, Tuple
+
+import torch
+import torch.distributed as dist
+from torch import Tensor
+
+from ..ops import cuda_ext
+from ..ops.dense import block_fwd
+from ..ops.merge import merge_partial
+from .comm import _wire, group_info
+from .ops import group_name, resolve_group
+
+KERNEL_HEAD_DIMS = (64, 128)  # the decode kernel is instantiated for these head sizes
+KEY_TILE = 128  # keys per K / V tile of the kernel
+ROWS_PER_CTA = 64  # packed (token, head-in-group) query rows per CTA
+
+
+@functools.lru_cache(maxsize=None)
+def _sm_count(index: int) -> int:
+    return torch.cuda.get_device_properties(index).multi_processor_count
+
+
+def num_splits(batch: int, sq: int, hq: int, hkv: int, s_cap: int, sm_count: int) -> int:
+    """Key-range splits per (sequence, kv head, row tile).  The kernel keeps one CTA per SM (its K/V ring fills the
+    shared memory), so the grid is sized to one full wave: more CTAs would leave a ragged second wave.  Derived from
+    shapes only, never from ``cache_seqlens``: splits past a sequence's valid keys exit at once, and nothing is read
+    back to the host (a decode step can be captured in a CUDA graph)."""
+    row_tiles = -(-sq * (hq // hkv) // ROWS_PER_CTA)
+    tiles = max(1, -(-s_cap // KEY_TILE))
+    return max(1, min(tiles, sm_count // (batch * hkv * row_tiles)))
+
+
+_warned = set()
+
+
+def _kernel_takes(q: Tensor) -> bool:
+    if not cuda_ext.available_for(q):
+        return False
+    if q.dtype in (torch.bfloat16, torch.float16) and q.shape[-1] in KERNEL_HEAD_DIMS:
+        return True
+    key = (q.dtype, q.shape[-1])
+    if key not in _warned:
+        _warned.add(key)
+        warnings.warn(f"cp_flash_attn_with_kvcache: no sm_90a decode kernel for {q.dtype} with head_dim {q.shape[-1]} "
+                      f"(instantiated: bf16 / fp16, head_dim {KERNEL_HEAD_DIMS}); running the dense torch path",
+                      RuntimeWarning, stacklevel=3)
+    return False
+
+
+def _gather(local: Tensor, pg, world: int) -> Tensor:
+    """(world, n) stack of every rank's flat fp32 partial, rank order, on the caller's stream."""
+    buf = local.new_empty(world * local.numel())  # flat: gloo takes only the concatenated form
+    dist.all_gather_into_tensor(_wire(buf), _wire(local), group=pg)
+    return buf.view(world, local.numel())
+
+
+# ----------------------------------------------------------------------------------------------
+# sm_90a path
+# ----------------------------------------------------------------------------------------------
+
+def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor, k: Optional[Tensor],
+                  v: Optional[Tensor], causal: bool, softmax_scale: float, pg=None, world: int = 1,
+                  splits: Optional[int] = None) -> Tuple[Tensor, Tensor]:
+    """Local split-KV kernel (appending ``k`` / ``v`` first when given), then the combine over the splits and, for
+    ``world > 1``, over the gathered per-rank partials.  ``splits`` overrides :func:`num_splits`."""
+    C = cuda_ext.load()
+    b, sq, hq, d = q.shape
+    q = q.contiguous()
+    if k is not None:
+        k, v = k.contiguous(), v.contiguous()
+    if splits is None:
+        dev = q.device.index if q.device.index is not None else torch.cuda.current_device()
+        splits = num_splits(b, sq, hq, k_cache.shape[2], k_cache.shape[1], _sm_count(dev))
+    n_out = b * sq * hq * d
+    size = n_out + b * hq * sq
+    parts = torch.empty((splits, size), dtype=torch.float32, device=q.device)
+    C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts)
+    cuda_ext.note_launch(2 if k is not None else 1)
+    if world > 1:
+        mine = torch.empty(size, dtype=torch.float32, device=q.device)
+        C.decode_combine(parts, mine[:n_out].view(b, sq, hq, d), mine[n_out:].view(b, hq, sq))
+        cuda_ext.note_launch()
+        parts = _gather(mine, pg, world)
+    out = torch.empty(q.shape, dtype=q.dtype, device=q.device)
+    lse = torch.empty((b, hq, sq), dtype=torch.float32, device=q.device)
+    C.decode_combine(parts, out, lse)
+    cuda_ext.note_launch()
+    return out, lse
+
+
+# ----------------------------------------------------------------------------------------------
+# dense path
+# ----------------------------------------------------------------------------------------------
+
+def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world):
+    b, sq, hq, d = q.shape
+    s_cap = k_cache.shape[1]
+    lens = [max(0, min(int(x), s_cap)) for x in cache_seqlens.tolist()]
+    n_new = sq if k is not None else 0
+    if k is not None:  # rows past the capacity are dropped, as in the kernel path
+        for i, n in enumerate(lens):
+            m = min(sq, s_cap - n)
+            k_cache[i, n:n + m] = k[i, :m]
+            v_cache[i, n:n + m] = v[i, :m]
+    out = torch.zeros((b, sq, hq, d), dtype=torch.float32, device=q.device)
+    lse = torch.full((b, hq, sq), float("-inf"), dtype=torch.float32, device=q.device)
+    for i, n in enumerate(lens):
+        n_keys = min(n + n_new, s_cap)
+        if n_keys == 0:
+            continue
+        # appended key u (row n + u) is visible to token t iff u <= t, i.e. row j <= t + n
+        diag = n if (n_new and causal) else None
+        out[i], lse[i] = block_fwd(q[i], k_cache[i, :n_keys], v_cache[i, :n_keys], softmax_scale, diag)
+    if world > 1:
+        parts = _gather(torch.cat([out.reshape(-1), lse.reshape(-1)]), pg, world)
+        n_out = out.numel()
+        acc_o = acc_l = None
+        for r in range(world):  # rank order: the same on every rank
+            o = parts[r, :n_out].view(b * sq, hq, d)
+            l = parts[r, n_out:].view(b, hq, sq).permute(1, 0, 2).reshape(hq, b * sq)
+            acc_o, acc_l = merge_partial(acc_o, acc_l, o, l)
+        out = acc_o.view(b, sq, hq, d)
+        lse = acc_l.view(hq, b, sq).permute(1, 0, 2).contiguous()
+    return out.to(q.dtype), lse
+
+
+# ----------------------------------------------------------------------------------------------
+# the op and the public function
+# ----------------------------------------------------------------------------------------------
+
+@torch.library.custom_op("rfa_b200::cp_decode", mutates_args=("k_cache", "v_cache"))
+def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor, k: Optional[Tensor],
+              v: Optional[Tensor], append_rank: int, softmax_scale: float, causal: bool,
+              group: str) -> Tuple[Tensor, Tensor]:
+    """q (B, Sq, Hq, D) -> (out (B, Sq, Hq, D) in q.dtype, lse (B, Hq, Sq) fp32).  ``k`` / ``v`` are appended to
+    the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's name ("" = world)."""
+    pg = resolve_group(group)
+    rank, world = group_info(pg)
+    if k is not None and not 0 <= append_rank < world:
+        raise ValueError(f"append_rank={append_rank} is not a rank of the {world}-rank group")
+    if rank != append_rank:
+        k = v = None
+    if _kernel_takes(q):
+        return kernel_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world)
+    return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world)
+
+
+@cp_decode.register_fake
+def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group):
+    b, sq, hq, _ = q.shape
+    return q.new_empty(q.shape), q.new_empty((b, hq, sq), dtype=torch.float32)
+
+
+def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=None, append_rank=None,
+                               softmax_scale=None, causal=True, return_softmax_lse=False, group=None, *,
+                               window_size=(-1, -1), alibi_slopes=None):
+    """Decode attention of new query tokens against a KV cache sharded over ``group`` (modelled on flash-attn's
+    ``flash_attn_with_kvcache``).  Inference only: no gradient.
+
+    * ``q`` ``(B, Sq, Hq, D)``, the same on every rank; ``Sq >= 1`` (one token, or a few speculative ones).
+    * ``k_cache`` / ``v_cache`` ``(B, S_cap, Hkv, D)``: this rank's shard, in any row order (the local K / V of a
+      ring / zigzag / stripe / llama3 / zigzag-llama3 prefill can be used as is).  Batch and sequence dimensions must
+      be mergeable (``stride(0) == S_cap * stride(1)``).
+    * ``cache_seqlens`` ``(B,)`` int32 on q's device: valid rows of this rank's shard (0 = empty shard).
+    * ``k`` / ``v`` ``(B, Sq, Hkv, D)``, optional, the same on every rank: written in place into the caches of rank
+      ``append_rank`` only, at rows ``[cache_seqlens[b], cache_seqlens[b] + Sq)``, before attention (rows past
+      ``S_cap`` are dropped).  The caller advances ``cache_seqlens``.  ``append_rank`` is required with ``k`` / ``v``
+      and must be ``None`` without them; it must be the same int on every rank (e.g. ``step % world``).
+    * Query token ``t`` sees every valid cached key of every rank and, with ``causal=True``, the appended keys
+      ``0..t`` of its own call (flash-attn's bottom-right alignment); with ``causal=False`` all ``Sq`` of them.
+    * Returns ``out`` ``(B, Sq, Hq, D)`` in q.dtype, and ``softmax_lse`` ``(B, Hq, Sq)`` fp32 when
+      ``return_softmax_lse``.  Both are bitwise identical on every rank.
+    * ``window_size``, ``alibi_slopes``, fp8 caches, ``D > 128`` and ``Hq % Hkv != 0`` raise ``ValueError``.  The
+      sm_90a kernel covers bf16 / fp16 with ``D`` in {64, 128}; other head sizes run the dense torch path with a
+      one-time warning.
+    * Nothing is read back to the host on the kernel path, so a decode step can be captured in a CUDA graph.
+
+    RoPE: the positions of the new tokens are the caller's to apply (prefill length plus the decode step)."""
+    if tuple(window_size) != (-1, -1):
+        raise ValueError("cp_flash_attn_with_kvcache: sliding windows are not supported in decode")
+    if alibi_slopes is not None:
+        raise ValueError("cp_flash_attn_with_kvcache: alibi_slopes are not supported in decode")
+    if q.dim() != 4 or k_cache.dim() != 4 or tuple(k_cache.shape) != tuple(v_cache.shape):
+        raise ValueError("q must be (B, Sq, Hq, D) and k_cache / v_cache the same (B, S_cap, Hkv, D) shape")
+    b, sq, hq, d = q.shape
+    hkv = k_cache.shape[2]
+    if k_cache.shape[0] != b or k_cache.shape[3] != d or sq < 1:
+        raise ValueError(f"q {tuple(q.shape)} does not match the cache {tuple(k_cache.shape)}")
+    if q.element_size() == 1 or k_cache.element_size() == 1 or v_cache.element_size() == 1:
+        raise ValueError("cp_flash_attn_with_kvcache: fp8 queries / caches are not supported")
+    if k_cache.dtype != q.dtype or v_cache.dtype != q.dtype:
+        raise ValueError("k_cache / v_cache must have q's dtype")
+    if d > 128:
+        raise ValueError(f"cp_flash_attn_with_kvcache: head_dim {d} > 128 is not supported")
+    if hq % hkv != 0:
+        raise ValueError(f"query heads ({hq}) must be a multiple of kv heads ({hkv})")
+    if (cache_seqlens.dtype != torch.int32 or tuple(cache_seqlens.shape) != (b,)
+            or cache_seqlens.device != q.device):
+        raise ValueError("cache_seqlens must be a (B,) int32 tensor on q's device")
+    if (k is None) != (v is None):
+        raise ValueError("pass both k and v, or neither")
+    if k is not None:
+        if append_rank is None:
+            raise ValueError("append_rank is required when k / v are given")
+        for t in (k, v):
+            if tuple(t.shape) != (b, sq, hkv, d) or t.dtype != q.dtype:
+                raise ValueError(f"k / v must be (B, Sq, Hkv, D) = {(b, sq, hkv, d)} in q's dtype")
+    elif append_rank is not None:
+        raise ValueError("append_rank must be None when no k / v are given")
+    scale = float(softmax_scale) if softmax_scale is not None else d ** -0.5
+    out, lse = cp_decode(q, k_cache, v_cache, cache_seqlens, k, v, -1 if append_rank is None else int(append_rank),
+                         scale, bool(causal), group_name(group))
+    return (out, lse) if return_softmax_lse else out

@@ -42,15 +42,17 @@ lines += ["All functions additionally accept the keyword-only `descale=` *(exten
           "* `window_size=(left, right)`: sliding window on global positions, every scheme; `-1` = unbounded.",
           "* `softmax_scale`: default `head_dim ** -0.5` of the unpadded head size.",
           "* `dropout_p`, `alibi_slopes`: must be `0.0` / `None` (`NotImplementedError` otherwise).",
-          "* `deterministic=True`: out / lse / dQ / dK / dV bitwise reproducible. On the sm_100a path the backward then",
+          "* `deterministic=True`: out / lse / dQ / dK / dV bitwise reproducible. On the sm_90a path the backward then",
           "  launches its key tiles in groups with disjoint query rows and, across GPUs, uses the fixed-order",
           "  torch.distributed transport (several times slower; a one-time `RuntimeWarning` says so).",
           "  `RFA_B200_DETERMINISTIC=fast` keeps the fused schedule: dK / dV reproducible, dQ an unordered fp32 sum.",
           "* `return_attn_probs=True`: returns `(out, softmax_lse, None)`; lse is fp32, `(B, H, S_local)` (batch) or",
           "  `(H, T_local)` (varlen).",
           "* `group`: the context-parallel process group (`None` = world). Every rank of the group must make the same",
-          "  calls in the same order: on B200s the launches contain the K/V exchange.",
+          "  calls in the same order: on H100s the launches contain the K/V exchange.",
           "* packed inputs (`qkv`, `kv`): sliced as views; their gradient is written as one concatenation.", ""]
+section("Decoding over a sharded KV cache (`ring_flash_attn_b200`, implemented in `parallel/decode.py`)")
+entry("cp_flash_attn_with_kvcache", rfa.cp_flash_attn_with_kvcache, ext=True)
 section("Hugging Face adapter (`ring_flash_attn_b200`, implemented in `models/hf_adapter.py`)")
 for n in ("substitute_hf_flash_attn", "update_ring_flash_attn_params", "use_ring_attn"):
     entry(n, getattr(hf_adapter, n))
