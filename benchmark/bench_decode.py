@@ -4,9 +4,12 @@ local shard, alternating in one run.
 One JSON line per (batch, cache length): device-timed microseconds per call, the K + V bytes the call must read, the
 achieved rate and its share of the H100 SXM data-sheet HBM bandwidth (3.35 TB/s; a data-sheet figure, not a measured
 peak), with the card name and power limit.  Under ``torchrun`` (world > 1) every rank holds a shard of that length and
-the line also reports the all-gather + combine time of the cross-rank merge.
+the line also reports the all-gather + combine time of the cross-rank merge.  With ``--page-size N`` every
+configuration also times the kernel on a paged copy of the same cache (pages in a seeded random order, one block
+table per sequence) in the same alternating loop, and reports whether its output is bitwise the contiguous one.
 
     python benchmark/bench_decode.py                      # B in {1, 8}, caches of 32K..512K tokens per rank
+    python benchmark/bench_decode.py --page-size 16       # also the paged kernel, pages of 16 rows
     torchrun --nproc-per-node 2 benchmark/bench_decode.py
     python benchmark/bench_decode.py --dry-run            # shapes and byte counts only (no GPU)
 """
@@ -36,6 +39,7 @@ def parse_args(argv=None):
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--sm-count", type=int, default=132, help="used by --dry-run only")
+    ap.add_argument("--page-size", type=int, default=None, help="also time a paged cache with pages of N rows")
     ap.add_argument("--dry-run", action="store_true")
     return ap.parse_args(argv)
 
@@ -44,9 +48,12 @@ def shapes(args, sm_count):
     """One dict per configuration: shapes, split count and the K + V bytes one call reads (bf16)."""
     for b in args.batch:
         for s in args.cache:
-            yield dict(batch=b, cache_tokens=s, sq=args.sq, hq=args.hq, hkv=args.hkv, head_dim=args.head_dim,
+            cfg = dict(batch=b, cache_tokens=s, sq=args.sq, hq=args.hq, hkv=args.hkv, head_dim=args.head_dim,
                        splits=dec.num_splits(b, args.sq, args.hq, args.hkv, s, sm_count),
                        kv_bytes=b * s * args.hkv * args.head_dim * 2 * 2)
+            if args.page_size:
+                cfg.update(page_size=args.page_size, block_table_bytes=b * -(-s // args.page_size) * 4)
+            yield cfg
 
 
 def card():
@@ -101,7 +108,23 @@ def main():
         scale = d ** -0.5
 
         def ours():
-            dec.kernel_decode(q, kc, vc, sl, None, None, True, scale)
+            return dec.kernel_decode(q, kc, vc, sl, None, None, True, scale)
+
+        if args.page_size:  # the same rows in a pool whose pages are in a seeded random order
+            ps = args.page_size
+            max_blocks = -(-s // ps)
+            perm = torch.randperm(b * max_blocks, generator=torch.Generator().manual_seed(rank)).to(dev)
+            table = perm.to(torch.int32).view(b, max_blocks)
+            pk = kc.new_zeros(b * max_blocks, ps, args.hkv, d)
+            pv = vc.new_zeros(b * max_blocks, ps, args.hkv, d)
+            for src, pool in ((kc, pk), (vc, pv)):
+                pad = src.new_zeros(b, max_blocks * ps, args.hkv, d)
+                pad[:, :s] = src
+                pool[perm.long()] = pad.view(b * max_blocks, ps, args.hkv, d)
+                del pad
+
+            def paged():
+                return dec.kernel_decode(q, pk, pv, sl, None, None, True, scale, block_table=table)
 
         # SDPA reads the same shard through (B, H, S, D) views
         qt, kt, vt = q.transpose(1, 2), kc.transpose(1, 2), vc.transpose(1, 2)
@@ -110,9 +133,13 @@ def main():
             F.scaled_dot_product_attention(qt, kt, vt, scale=scale, enable_gqa=True)
 
         rows = {"ours": [], "sdpa": []}
+        if args.page_size:
+            rows["paged"] = []
         sdpa_err = None
-        for _ in range(3):  # alternate the two in one run
+        for _ in range(3):  # alternate them in one run
             rows["ours"].append(time_us(ours, args.iters, args.warmup))
+            if args.page_size:
+                rows["paged"].append(time_us(paged, args.iters, args.warmup))
             if sdpa_err is None:
                 try:
                     rows["sdpa"].append(time_us(sdpa, args.iters, args.warmup))
@@ -129,6 +156,8 @@ def main():
                 res[f"{k}_share_of_datasheet_hbm"] = round(cfg["kv_bytes"] / (us * 1e-6) / HBM_DATASHEET_BPS, 3)
         if sdpa_err:
             res["sdpa_error"] = sdpa_err
+        if args.page_size:
+            res["paged_equal_contiguous"] = all(torch.equal(x, y) for x, y in zip(paged(), ours()))
         if world > 1:
             C = dec.cuda_ext.load()
             n_out = b * args.sq * args.hq * d
@@ -146,6 +175,8 @@ def main():
         if rank == 0:
             print(json.dumps(res), flush=True)
         del q, kc, vc
+        if args.page_size:
+            del pk, pv
         torch.cuda.empty_cache()
     if world > 1:
         dist.destroy_process_group()

@@ -399,25 +399,41 @@ at::Tensor lse_unflatten(const at::Tensor& lse, const at::Tensor& cu, int64_t ma
 
 // Split-KV decode (csrc/decode_sm90.cu).  q (B, Sq, Hq, D); k_cache / v_cache (B, S_cap, Hkv, D) with mergeable
 // batch and sequence dimensions; seqlens (B,) int32; k_new / v_new (B, Sq, Hkv, D) contiguous, appended to the caches
-// before attention when given.  part: fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq), see DecodeParams.
+// before attention when given.  part: fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq), see DecodeParams.  With block_table
+// (B, max_blocks) int32, the caches are page pools (num_blocks, page_size, Hkv, D) with mergeable page and row
+// dimensions, and S_cap = max_blocks * page_size.
 void decode_fwd(const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
                 const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
-                double scale, at::Tensor& part) {
+                double scale, at::Tensor& part, const c10::optional<at::Tensor>& block_table) {
   const c10::cuda::CUDAGuard guard(q.device());
   TORCH_CHECK(q.dim() == 4 && k_cache.dim() == 4 && v_cache.dim() == 4, "decode_fwd: 4-D q / k_cache / v_cache");
   TORCH_CHECK(k_cache.sizes() == v_cache.sizes(), "decode_fwd: k_cache and v_cache shapes differ");
   TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(),
               "decode_fwd: caches must have q's dtype");
   const int64_t B = q.size(0), sq = q.size(1), hq = q.size(2), d = q.size(3);
-  const int64_t s_cap = k_cache.size(1), hkv = k_cache.size(2);
-  TORCH_CHECK(k_cache.size(0) == B && k_cache.size(3) == d, "decode_fwd: cache shape does not match q");
+  const bool paged = block_table.has_value();
+  const int64_t page_size = paged ? k_cache.size(1) : 0;
+  const int64_t s_cap = paged ? block_table->size(1) * page_size : k_cache.size(1);
+  const int64_t hkv = k_cache.size(2);
+  const int64_t cache_rows = k_cache.size(0) * k_cache.size(1);
+  TORCH_CHECK((paged || k_cache.size(0) == B) && k_cache.size(3) == d, "decode_fwd: cache shape does not match q");
   TORCH_CHECK(q.stride(3) == 1 && q.stride(0) == sq * q.stride(1), "decode_fwd: q must be (B, Sq) mergeable");
   TORCH_CHECK((q.stride(1) * 2) % 16 == 0 && (q.stride(2) * 2) % 16 == 0 &&
                   reinterpret_cast<uintptr_t>(q.data_ptr()) % 16 == 0,
               "decode_fwd: q rows must be 16-byte aligned");
   for (const at::Tensor* c : {&k_cache, &v_cache})
-    TORCH_CHECK(c->stride(3) == 1 && c->stride(0) == s_cap * c->stride(1),
-                "decode_fwd: the cache's batch and sequence dimensions must be mergeable (stride(0) == S_cap * stride(1))");
+    TORCH_CHECK(c->stride(3) == 1 && c->stride(0) == c->size(1) * c->stride(1),
+                "decode_fwd: the cache's first two dimensions must be mergeable (stride(0) == size(1) * stride(1))");
+  if (paged) {
+    const at::Tensor& bt = *block_table;
+    TORCH_CHECK(bt.scalar_type() == at::kInt && bt.is_cuda() && bt.device() == q.device() && bt.dim() == 2 &&
+                    bt.size(0) == B && bt.size(1) >= 1 && bt.stride(1) == 1,
+                "decode_fwd: block_table must be (B, max_blocks) int32 on q's device with stride(1) == 1");
+    TORCH_CHECK(page_size == 16 || page_size == 32 || page_size == 64 || (page_size > 0 && page_size % 128 == 0),
+                "decode_fwd: page_size must be 16, 32, 64 or a positive multiple of 128");
+    TORCH_CHECK(cache_rows < (int64_t(1) << 31) && s_cap < (int64_t(1) << 31),
+                "decode_fwd: num_blocks * page_size and max_blocks * page_size must be below 2^31");
+  }
   TORCH_CHECK(seqlens.scalar_type() == at::kInt && seqlens.is_cuda() && seqlens.is_contiguous() && seqlens.numel() == B,
               "decode_fwd: cache_seqlens must be (B,) int32 on the device");
   TORCH_CHECK(part.scalar_type() == at::kFloat && part.is_contiguous() && part.dim() == 2 && part.size(0) >= 1 &&
@@ -452,8 +468,14 @@ void decode_fwd(const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, c
   p.n_new = kn != nullptr ? static_cast<int>(sq) : 0;
   p.causal = causal ? 1 : 0;
   p.scale_log2 = static_cast<float>(scale * 1.4426950408889634);
-  const TensorView kv{k_cache.data_ptr(), B * s_cap, static_cast<int>(hkv), k_cache.stride(1), k_cache.stride(2)};
-  const TensorView vv{v_cache.data_ptr(), B * s_cap, static_cast<int>(hkv), v_cache.stride(1), v_cache.stride(2)};
+  if (paged) {
+    p.block_table = block_table->data_ptr<int>();
+    p.bt_stride = block_table->stride(0);
+    p.page_size = static_cast<int>(page_size);
+    p.num_pages = static_cast<int>(k_cache.size(0));
+  }
+  const TensorView kv{k_cache.data_ptr(), cache_rows, static_cast<int>(hkv), k_cache.stride(1), k_cache.stride(2)};
+  const TensorView vv{v_cache.data_ptr(), cache_rows, static_cast<int>(hkv), v_cache.stride(1), v_cache.stride(2)};
   check(rfa::decode_fwd_launch(dtype_code(q), kv, vv, kn, vn, p, static_cast<int>(n_splits), static_cast<int>(d),
                                at::cuda::getCurrentCUDAStream()));
 }

@@ -22,10 +22,17 @@ struct DecodeParams {
   int n_new;               // keys appended to this shard by this call (0 on every rank but the append rank)
   int causal;              // appended key u is visible to query token t only if u <= t
   float scale_log2;        // softmax scale * log2(e)
+  // Paged caches: logical row j of sequence b is row j % page_size of page block_table[b * bt_stride + j / page_size]
+  // of a pool of num_pages pages; the tensor maps then cover the (num_pages * page_size, Hkv, D) view of the pool.
+  const int* block_table;  // nullptr when page_size == 0
+  long long bt_stride;     // table entries between consecutive sequences
+  int page_size;           // 0: contiguous (B, S_cap, Hkv, D) caches; else 16, 32, 64 or a multiple of 128
+  int num_pages;
 };
 
 // Appends k_new / v_new (B, Sq, Hkv, D), contiguous, at rows [seqlens[b], seqlens[b] + Sq) of the caches (rows past
-// the capacity are dropped), then runs the split-KV kernel.  k_new == nullptr: attention only.
+// the capacity, and with a block table rows whose page id is outside the pool, are dropped), then runs the split-KV
+// kernel.  k_new == nullptr: attention only.
 const char* decode_fwd_launch(int dtype, const TensorView& k_cache, const TensorView& v_cache, const void* k_new,
                               const void* v_new, const DecodeParams& p, int n_splits, int head_dim,
                               cudaStream_t stream);

@@ -49,6 +49,67 @@ __device__ __forceinline__ int key_limit(const DecodeParams& p, int seqlen, int 
   return lim < p.s_cap ? lim : p.s_cap;
 }
 
+// TMA producer over a paged cache, run by the whole producer warp.  A 128-key tile is one page (page_size >= 128,
+// the tile starts at row key0 % page_size of it) or 128 / page_size pages, each loaded as its own box of page_size
+// rows into the matching rows of the slot: an offset of i * page_size * 128 bytes stays 1024-byte aligned, so the
+// 128-byte swizzle is the one a single 128-row box writes.  Pages past the last visible key (kmax) are neither
+// looked up nor loaded, and neither are pages whose id lies outside the pool (a caller error); the slot's expected
+// byte count covers only the boxes issued.  The rows left unwritten hold an older tile, and the compute warpgroup
+// already discards every row at or past kmax (K columns masked, V rows zeroed), exactly as for a contiguous cache.
+// Table entries are read 32 at a time, one per lane, a window ahead of use, and broadcast with shuffles.
+template <int kD>
+__device__ __forceinline__ void produce_paged(const CUtensorMap* tm_k, const CUtensorMap* tm_v, Barriers* bars,
+                                              uint8_t* smem_kv, const DecodeParams& p, int b, int kv_head, int j0,
+                                              int n_tiles, int kmax) {
+  constexpr int kSubTiles = kD / 64;
+  constexpr int kSlotBytes = kTile * kD * 2;
+  const int lane = threadIdx.x & 31;
+  const int ps = p.page_size;
+  const int box = ps < kTile ? ps : kTile;  // rows per TMA box, as in the tensor maps
+  const int n_sub = kTile / box;            // pages per tile: 8, 4, 2 or 1
+  const int* table = p.block_table + b * p.bt_stride;
+  const int last = (kmax - 1) / ps;  // last page holding a visible key; later entries are never read
+  auto entry = [&](int i) { return i <= last ? __ldg(table + i) : -1; };
+  int win = j0 * kTile / ps;  // first page of the split; cur holds table entries [win, win + 32), nxt the next 32
+  int cur = entry(win + lane), nxt = entry(win + 32 + lane);
+  uint32_t slot = 0, phase = 0;
+  for (int jj = 0; jj < n_tiles; ++jj) {
+    const int key0 = (j0 + jj) * kTile;
+    const int pg0 = key0 / ps;  // first page of the tile
+    if (pg0 - win >= 32) {      // n_sub divides 32 and win starts at a tile's first page: a tile never straddles
+      win += 32;
+      cur = nxt;
+      nxt = entry(win + 32 + lane);
+    }
+    // lane i < n_sub: sub-tile i, i.e. keys [key0 + i * box, key0 + (i + 1) * box)
+    const int page = __shfl_sync(0xffffffffu, cur, (pg0 - win + lane) & 31);
+    const bool live = lane < n_sub && key0 + lane * box < kmax && page >= 0 && page < p.num_pages;
+    const int row = live ? page * ps + (key0 - pg0 * ps) : 0;
+    const unsigned loads = __ballot_sync(0xffffffffu, live);
+    const uint32_t tx = __popc(loads) * box * 128 * kSubTiles;
+    for (int kv = 0; kv < 2; ++kv) {
+      uint8_t* dst = smem_kv + slot * kSlotBytes;
+      if (lane == 0) {
+        mbar_wait(&bars->kv_empty[slot], phase ^ 1);
+        mbar_arrive_expect_tx(&bars->kv_full[slot], tx);
+      }
+      for (int i = 0; i < n_sub; ++i) {
+        const int r = __shfl_sync(0xffffffffu, row, i);
+        if (lane == 0 && (loads >> i & 1u)) {
+#pragma unroll
+          for (int h = 0; h < kSubTiles; ++h)
+            tma_load_3d(dst + h * kKHalfBytes + i * box * 128, kv == 0 ? tm_k : tm_v, &bars->kv_full[slot], 64 * h,
+                        kv_head, r);
+        }
+      }
+      if (++slot == kStages) {
+        slot = 0;
+        phase ^= 1;
+      }
+    }
+  }
+}
+
 template <typename T, int kD>
 __global__ void __launch_bounds__(kThreads, 1)
 decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
@@ -91,7 +152,9 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
 
   if (threadIdx.x >= 128) {
     // ------------------------------------------------------------------ TMA producer
-    if (threadIdx.x == 128) {
+    if (p.page_size != 0) {
+      if (n_tiles > 0) produce_paged<kD>(&tm_k, &tm_v, bars, smem_kv, p, b, kv_head, j0, n_tiles, kmax);
+    } else if (threadIdx.x == 128) {
       uint32_t slot = 0, phase = 0;
       for (int jj = 0; jj < n_tiles; ++jj) {
         const int row = b * p.s_cap + (j0 + jj) * kTile;  // rows past the tensor's end arrive as zeros
@@ -283,14 +346,21 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
 }
 
 // One block per (b, t) row of the new keys, blockIdx.y selects K or V.  16-byte chunks; rows past the capacity
-// are dropped.
+// are dropped, and so are rows whose page id lies outside the pool.
 __global__ void decode_append_kernel(uint8_t* k_cache, uint8_t* v_cache, long long row_stride_bytes,
                                      long long head_stride_bytes, const uint8_t* k_new, const uint8_t* v_new,
-                                     const int* seqlens, int sq, int hkv, int row_bytes, int s_cap) {
+                                     const DecodeParams p, int row_bytes) {
+  const int sq = p.sq, hkv = p.hkv;
   const int b = blockIdx.x / sq, t = blockIdx.x % sq;
-  const int row = seqlens[b] + t;
-  if (row < 0 || row >= s_cap) return;
-  uint8_t* dst = (blockIdx.y == 0 ? k_cache : v_cache) + (static_cast<long long>(b) * s_cap + row) * row_stride_bytes;
+  const int row = p.seqlens[b] + t;
+  if (row < 0 || row >= p.s_cap) return;
+  long long cache_row = static_cast<long long>(b) * p.s_cap + row;
+  if (p.page_size != 0) {
+    const int page = p.block_table[b * p.bt_stride + row / p.page_size];
+    if (page < 0 || page >= p.num_pages) return;
+    cache_row = static_cast<long long>(page) * p.page_size + row % p.page_size;
+  }
+  uint8_t* dst = (blockIdx.y == 0 ? k_cache : v_cache) + cache_row * row_stride_bytes;
   const uint8_t* src = (blockIdx.y == 0 ? k_new : v_new) + static_cast<long long>(blockIdx.x) * hkv * row_bytes;
   const int chunks = row_bytes / 16;
   for (int idx = threadIdx.x; idx < hkv * chunks; idx += blockDim.x) {
@@ -352,14 +422,22 @@ const char* decode_fwd_launch(int dtype, const TensorView& k_cache, const Tensor
   if (p.hkv <= 0 || p.hq % p.hkv != 0) return "query heads must be a multiple of kv heads";
   if (k_cache.row_stride != v_cache.row_stride || k_cache.head_stride != v_cache.head_stride)
     return "k_cache and v_cache must have the same strides";
+  if (p.page_size != 0) {
+    const bool size_ok = p.page_size == 16 || p.page_size == 32 || p.page_size == 64 ||
+                         (p.page_size > 0 && p.page_size % dec::kTile == 0);
+    if (!size_ok) return "page_size must be 16, 32, 64 or a positive multiple of 128";
+    if (p.block_table == nullptr) return "a paged cache needs a block table";
+  }
+  // a paged cache's tensor maps cover the whole pool; a box is at most one page
+  const int box_rows = p.page_size != 0 && p.page_size < dec::kTile ? p.page_size : dec::kTile;
   CUtensorMap tk, tv;
-  if (const char* e = make_tensor_map(&tk, k_cache, 2, dec::kTile, head_dim)) return e;
-  if (const char* e = make_tensor_map(&tv, v_cache, 2, dec::kTile, head_dim)) return e;
+  if (const char* e = make_tensor_map(&tk, k_cache, 2, box_rows, head_dim)) return e;
+  if (const char* e = make_tensor_map(&tv, v_cache, 2, box_rows, head_dim)) return e;
   if (k_new != nullptr && p.n_new > 0) {
     dec::decode_append_kernel<<<dim3(p.batch * p.sq, 2), 128, 0, stream>>>(
         static_cast<uint8_t*>(k_cache.ptr), static_cast<uint8_t*>(v_cache.ptr), k_cache.row_stride * 2,
-        k_cache.head_stride * 2, static_cast<const uint8_t*>(k_new), static_cast<const uint8_t*>(v_new), p.seqlens,
-        p.sq, p.hkv, head_dim * 2, p.s_cap);
+        k_cache.head_stride * 2, static_cast<const uint8_t*>(k_new), static_cast<const uint8_t*>(v_new), p,
+        head_dim * 2);
   }
   const int row_tiles = (p.sq * (p.hq / p.hkv) + dec::kRows - 1) / dec::kRows;
   dim3 grid(n_splits, row_tiles, p.batch * p.hkv), block(dec::kThreads, 1, 1);

@@ -79,11 +79,17 @@ def _gather(local: Tensor, pg, world: int) -> Tensor:
 # sm_90a path
 # ----------------------------------------------------------------------------------------------
 
+def _capacity(k_cache: Tensor, block_table: Optional[Tensor]) -> int:
+    """Cache rows per sequence: ``S_cap``, or ``max_blocks * page_size`` for a paged cache."""
+    return k_cache.shape[1] if block_table is None else block_table.shape[1] * k_cache.shape[1]
+
+
 def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor, k: Optional[Tensor],
                   v: Optional[Tensor], causal: bool, softmax_scale: float, pg=None, world: int = 1,
-                  splits: Optional[int] = None) -> Tuple[Tensor, Tensor]:
+                  splits: Optional[int] = None, block_table: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
     """Local split-KV kernel (appending ``k`` / ``v`` first when given), then the combine over the splits and, for
-    ``world > 1``, over the gathered per-rank partials.  ``splits`` overrides :func:`num_splits`."""
+    ``world > 1``, over the gathered per-rank partials.  ``splits`` overrides :func:`num_splits`.  With
+    ``block_table`` the caches are page pools (see :func:`cp_flash_attn_with_kvcache`)."""
     C = cuda_ext.load()
     b, sq, hq, d = q.shape
     q = q.contiguous()
@@ -91,11 +97,11 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
         k, v = k.contiguous(), v.contiguous()
     if splits is None:
         dev = q.device.index if q.device.index is not None else torch.cuda.current_device()
-        splits = num_splits(b, sq, hq, k_cache.shape[2], k_cache.shape[1], _sm_count(dev))
+        splits = num_splits(b, sq, hq, k_cache.shape[2], _capacity(k_cache, block_table), _sm_count(dev))
     n_out = b * sq * hq * d
     size = n_out + b * hq * sq
     parts = torch.empty((splits, size), dtype=torch.float32, device=q.device)
-    C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts)
+    C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts, block_table)
     cuda_ext.note_launch(2 if k is not None else 1)
     if world > 1:
         mine = torch.empty(size, dtype=torch.float32, device=q.device)
@@ -113,25 +119,41 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
 # dense path
 # ----------------------------------------------------------------------------------------------
 
-def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world):
+def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table=None):
     b, sq, hq, d = q.shape
-    s_cap = k_cache.shape[1]
+    s_cap = _capacity(k_cache, block_table)
     lens = [max(0, min(int(x), s_cap)) for x in cache_seqlens.tolist()]
     n_new = sq if k is not None else 0
-    if k is not None:  # rows past the capacity are dropped, as in the kernel path
+    ps, n_pages = k_cache.shape[1], k_cache.shape[0]
+    table = block_table.tolist() if block_table is not None else None
+    if k is not None:  # rows past the capacity (or whose page is outside the pool) are dropped, as in the kernel path
         for i, n in enumerate(lens):
             m = min(sq, s_cap - n)
-            k_cache[i, n:n + m] = k[i, :m]
-            v_cache[i, n:n + m] = v[i, :m]
+            if table is None:
+                k_cache[i, n:n + m] = k[i, :m]
+                v_cache[i, n:n + m] = v[i, :m]
+                continue
+            for t in range(m):
+                page = table[i][(n + t) // ps]
+                if 0 <= page < n_pages:
+                    k_cache[page, (n + t) % ps] = k[i, t]
+                    v_cache[page, (n + t) % ps] = v[i, t]
     out = torch.zeros((b, sq, hq, d), dtype=torch.float32, device=q.device)
     lse = torch.full((b, hq, sq), float("-inf"), dtype=torch.float32, device=q.device)
     for i, n in enumerate(lens):
         n_keys = min(n + n_new, s_cap)
         if n_keys == 0:
             continue
+        if table is None:
+            kk, vv = k_cache[i, :n_keys], v_cache[i, :n_keys]
+        else:  # the pages holding the visible rows, in table order
+            pages = table[i][:-(-n_keys // ps)]
+            if not all(0 <= x < n_pages for x in pages):
+                raise ValueError(f"block_table[{i}] points outside the {n_pages}-page pool for a page it reads")
+            kk, vv = k_cache[pages].flatten(0, 1)[:n_keys], v_cache[pages].flatten(0, 1)[:n_keys]
         # appended key u (row n + u) is visible to token t iff u <= t, i.e. row j <= t + n
         diag = n if (n_new and causal) else None
-        out[i], lse[i] = block_fwd(q[i], k_cache[i, :n_keys], v_cache[i, :n_keys], softmax_scale, diag)
+        out[i], lse[i] = block_fwd(q[i], kk, vv, softmax_scale, diag)
     if world > 1:
         parts = _gather(torch.cat([out.reshape(-1), lse.reshape(-1)]), pg, world)
         n_out = out.numel()
@@ -151,10 +173,11 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
 
 @torch.library.custom_op("rfa_b200::cp_decode", mutates_args=("k_cache", "v_cache"))
 def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor, k: Optional[Tensor],
-              v: Optional[Tensor], append_rank: int, softmax_scale: float, causal: bool,
-              group: str) -> Tuple[Tensor, Tensor]:
+              v: Optional[Tensor], append_rank: int, softmax_scale: float, causal: bool, group: str,
+              block_table: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
     """q (B, Sq, Hq, D) -> (out (B, Sq, Hq, D) in q.dtype, lse (B, Hq, Sq) fp32).  ``k`` / ``v`` are appended to
-    the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's name ("" = world)."""
+    the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's name ("" = world);
+    with ``block_table`` the caches are this rank's page pools."""
     pg = resolve_group(group)
     rank, world = group_info(pg)
     if k is not None and not 0 <= append_rank < world:
@@ -162,19 +185,41 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
     if rank != append_rank:
         k = v = None
     if _kernel_takes(q):
-        return kernel_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world)
-    return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world)
+        return kernel_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world,
+                             block_table=block_table)
+    return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table)
 
 
 @cp_decode.register_fake
-def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group):
+def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group, block_table):
     b, sq, hq, _ = q.shape
     return q.new_empty(q.shape), q.new_empty((b, hq, sq), dtype=torch.float32)
 
 
+def _valid_page_size(ps: int) -> bool:
+    return ps in (16, 32, 64) or (ps > 0 and ps % KEY_TILE == 0)
+
+
+def _check_block_table(q, k_cache, v_cache, block_table):
+    b = q.shape[0]
+    if (block_table.dtype != torch.int32 or block_table.dim() != 2 or block_table.shape[0] != b
+            or block_table.shape[1] < 1 or block_table.stride(1) != 1):
+        raise ValueError("block_table must be a (B, max_blocks) int32 tensor with stride(1) == 1")
+    if block_table.device != q.device:
+        raise ValueError("block_table must be on q's device")
+    n_blocks, ps = k_cache.shape[:2]
+    if not _valid_page_size(ps):
+        raise ValueError(f"page_size {ps} is not supported: use 16, 32, 64 or a positive multiple of 128")
+    for c in (k_cache, v_cache):
+        if c.stride(0) != ps * c.stride(1) or c.stride(3) != 1:
+            raise ValueError("the page pools must be mergeable: stride(0) == page_size * stride(1), stride(3) == 1")
+    if n_blocks * ps >= 2 ** 31 or block_table.shape[1] * ps >= 2 ** 31:
+        raise ValueError("num_blocks * page_size and max_blocks * page_size must be below 2^31")
+
+
 def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=None, append_rank=None,
                                softmax_scale=None, causal=True, return_softmax_lse=False, group=None, *,
-                               window_size=(-1, -1), alibi_slopes=None):
+                               block_table=None, window_size=(-1, -1), alibi_slopes=None):
     """Decode attention of new query tokens against a KV cache sharded over ``group`` (modelled on flash-attn's
     ``flash_attn_with_kvcache``).  Inference only: no gradient.
 
@@ -182,6 +227,15 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
     * ``k_cache`` / ``v_cache`` ``(B, S_cap, Hkv, D)``: this rank's shard, in any row order (the local K / V of a
       ring / zigzag / stripe / llama3 / zigzag-llama3 prefill can be used as is).  Batch and sequence dimensions must
       be mergeable (``stride(0) == S_cap * stride(1)``).
+    * ``block_table`` ``(B, max_blocks)`` int32 on q's device (``stride(1) == 1``), optional: the cache is paged.
+      ``k_cache`` / ``v_cache`` are then this rank's page pool ``(num_blocks, page_size, Hkv, D)``, with
+      ``stride(0) == page_size * stride(1)``, and row ``j`` of sequence ``b`` lives at row ``j % page_size`` of page
+      ``block_table[b, j // page_size]``.  Each rank has its own pool and table.  ``S_cap`` is
+      ``max_blocks * page_size``; ``page_size`` is 16, 32, 64 or a positive multiple of 128, and
+      ``num_blocks * page_size < 2**31``.  Entries of pages that hold no visible row are never read (-1 is fine).
+      On the append rank the caller allocates the pages of rows ``[0, cache_seqlens[b] + Sq)`` before the call.
+      An entry outside the pool for a page that is read is a caller error: the kernel's result is then undefined,
+      but it never accesses memory outside the pool (the dense path raises ``ValueError``).
     * ``cache_seqlens`` ``(B,)`` int32 on q's device: valid rows of this rank's shard (0 = empty shard).
     * ``k`` / ``v`` ``(B, Sq, Hkv, D)``, optional, the same on every rank: written in place into the caches of rank
       ``append_rank`` only, at rows ``[cache_seqlens[b], cache_seqlens[b] + Sq)``, before attention (rows past
@@ -205,7 +259,7 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
         raise ValueError("q must be (B, Sq, Hq, D) and k_cache / v_cache the same (B, S_cap, Hkv, D) shape")
     b, sq, hq, d = q.shape
     hkv = k_cache.shape[2]
-    if k_cache.shape[0] != b or k_cache.shape[3] != d or sq < 1:
+    if (block_table is None and k_cache.shape[0] != b) or k_cache.shape[3] != d or sq < 1:
         raise ValueError(f"q {tuple(q.shape)} does not match the cache {tuple(k_cache.shape)}")
     if q.element_size() == 1 or k_cache.element_size() == 1 or v_cache.element_size() == 1:
         raise ValueError("cp_flash_attn_with_kvcache: fp8 queries / caches are not supported")
@@ -218,6 +272,8 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
     if (cache_seqlens.dtype != torch.int32 or tuple(cache_seqlens.shape) != (b,)
             or cache_seqlens.device != q.device):
         raise ValueError("cache_seqlens must be a (B,) int32 tensor on q's device")
+    if block_table is not None:
+        _check_block_table(q, k_cache, v_cache, block_table)
     if (k is None) != (v is None):
         raise ValueError("pass both k and v, or neither")
     if k is not None:
@@ -230,5 +286,5 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
         raise ValueError("append_rank must be None when no k / v are given")
     scale = float(softmax_scale) if softmax_scale is not None else d ** -0.5
     out, lse = cp_decode(q, k_cache, v_cache, cache_seqlens, k, v, -1 if append_rank is None else int(append_rank),
-                         scale, bool(causal), group_name(group))
+                         scale, bool(causal), group_name(group), block_table)
     return (out, lse) if return_softmax_lse else out
