@@ -26,6 +26,19 @@ class FakeExt:
     def __init__(self):
         self.calls = []
 
+    # the pieces of the contract that tests/test_kernel_oracle_cpu.py mutates
+    def _mask(self, n_rows, q_off, kv_len, diag, lo):
+        return _visible(n_rows, q_off, kv_len, diag, lo)
+
+    def _kv_heads(self, x, rep):  # query head h reads kv head h // rep
+        return x.repeat_interleave(rep, dim=1)
+
+    def _p_for_pv(self, p, dtype):  # P as the P V product sees it
+        return p
+
+    def _group_sum(self, x, hkv, rep):  # dK / dV of a kv head: sum over its query heads
+        return x.view(x.shape[0], hkv, rep, x.shape[2]).sum(2)
+
     # ------------------------------------------------------------------ forward
     def _fwd(self, q, k, v, items, segs, seg_lo, out, lse, scale, sqk=None, sv=None):
         hq, hkv = q.shape[1], k.shape[1]
@@ -37,9 +50,9 @@ class FakeExt:
             for si in range(seg_begin, seg_begin + seg_count):
                 kv_row0, kv_len, diag, _flag = segs[si]
                 lo = LO_NONE if seg_lo is None else int(seg_lo[si])
-                m = _visible(n_rows, q_off, kv_len, diag, lo)  # (n, kv_len)
-                kk = kf[kv_row0:kv_row0 + kv_len].repeat_interleave(rep, dim=1)  # (kv_len, hq, d)
-                vv = vf[kv_row0:kv_row0 + kv_len].repeat_interleave(rep, dim=1)
+                m = self._mask(n_rows, q_off, kv_len, diag, lo)  # (n, kv_len)
+                kk = self._kv_heads(kf[kv_row0:kv_row0 + kv_len], rep)  # (kv_len, hq, d)
+                vv = self._kv_heads(vf[kv_row0:kv_row0 + kv_len], rep)
                 s = torch.einsum("nhd,khd->hnk", qf[q_row0:q_row0 + n_rows], kk) * scale
                 if sqk is not None:
                     s = s * sqk.view(-1, 1, 1)
@@ -50,7 +63,7 @@ class FakeExt:
             l = torch.logsumexp(s, dim=-1)  # (hq, n)
             p = torch.exp(s - torch.where(torch.isinf(l), torch.zeros_like(l), l).unsqueeze(-1))
             p = torch.where(torch.isinf(s), torch.zeros_like(p), p)
-            o = torch.einsum("hnk,khd->nhd", p, vv)
+            o = torch.einsum("hnk,khd->nhd", self._p_for_pv(p, out.dtype), vv)
             if sv is not None:
                 o = o * sv.repeat_interleave(rep).view(1, -1, 1)
             out[q_row0:q_row0 + n_rows] = o.to(out.dtype)
@@ -92,25 +105,24 @@ class FakeExt:
         qf, dof, kf, vf = q.float(), dout.float(), k.float(), v.float()
         qsegs = qsegs.tolist()
         for kv_row0, kv_rows, seg_begin, seg_count, *_ in items.tolist():
-            kt = kf[kv_row0:kv_row0 + kv_rows].repeat_interleave(rep, dim=1)  # (kr, hq, d)
-            vt = vf[kv_row0:kv_row0 + kv_rows].repeat_interleave(rep, dim=1)
+            kt = self._kv_heads(kf[kv_row0:kv_row0 + kv_rows], rep)  # (kr, hq, d)
+            vt = self._kv_heads(vf[kv_row0:kv_row0 + kv_rows], rep)
             dk_t = torch.zeros(kv_rows, hq, q.shape[2])
             dv_t = torch.zeros(kv_rows, hq, q.shape[2])
             for q_row0, q_len, diag, lo in qsegs[seg_begin:seg_begin + seg_count]:
                 rows = slice(q_row0, q_row0 + q_len)
-                m = _visible(q_len, 0, kv_rows, diag, lo if window else LO_NONE)
+                m = self._mask(q_len, 0, kv_rows, diag, lo if window else LO_NONE)
                 s = torch.einsum("nhd,khd->hnk", qf[rows], kt) * scale
                 lr = lse[:, rows]
                 p = torch.exp(s - torch.where(torch.isinf(lr), torch.full_like(lr, float("inf")), lr).unsqueeze(-1))
                 p = p.masked_fill(~m.unsqueeze(0), 0.0)
-                dv_t += torch.einsum("hnk,nhd->khd", p, dof[rows])
+                dv_t += torch.einsum("hnk,nhd->khd", self._p_for_pv(p, q.dtype), dof[rows])
                 dp = torch.einsum("nhd,khd->hnk", dof[rows], vt)
                 ds = p * (dp - delta[:, rows].unsqueeze(-1)) * scale
                 dk_t += torch.einsum("hnk,nhd->khd", ds, qf[rows])
                 dq[rows] += torch.einsum("hnk,khd->nhd", ds, kt)
-            d = q.shape[2]
-            dk[kv_row0:kv_row0 + kv_rows] = dk_t.view(kv_rows, hkv, rep, d).sum(2)  # written, not accumulated
-            dv[kv_row0:kv_row0 + kv_rows] = dv_t.view(kv_rows, hkv, rep, d).sum(2)
+            dk[kv_row0:kv_row0 + kv_rows] = self._group_sum(dk_t, hkv, rep)  # written, not accumulated
+            dv[kv_row0:kv_row0 + kv_rows] = self._group_sum(dv_t, hkv, rep)
 
     def dq_finalize(self, acc, out):
         self.calls.append("dq_finalize")

@@ -25,7 +25,7 @@ def _close(got, want, name, rel=5e-2, abs_=2e-2):
     assert err < lim, f"{name}: max err {err} > {lim}"
 
 
-def _batch_case(rank, world, scheme, causal, p2p, hq, hkv, s_local, iters, d=128):
+def _batch_case(rank, world, scheme, causal, p2p, hq, hkv, s_local, iters, d=128, dtype=torch.bfloat16):
     os.environ["RFA_B200_DISABLE_P2P"] = "0" if p2p else "1"
     dev = torch.device("cuda", rank)
     torch.manual_seed(0)
@@ -36,7 +36,7 @@ def _batch_case(rank, world, scheme, causal, p2p, hq, hkv, s_local, iters, d=128
     dout = torch.randn(1, s, hq, d, device=dev)
     for t in (q, k, v, dout):
         dist.broadcast(t, src=0)
-    q, k, v, dout = (t.to(torch.bfloat16) for t in (q, k, v, dout))
+    q, k, v, dout = (t.to(dtype) for t in (q, k, v, dout))
     rq, rk, rv = (t.float().requires_grad_(True) for t in (q, k, v))
     ref_out, ref_lse = attention_oracle(rq, rk, rv, causal)
     ref_out.backward(dout.float())
@@ -64,6 +64,8 @@ def _all_batch_cases(rank, world, p2p):
     for scheme, causal, hq, hkv, s_local in BATCH_CASES:
         _batch_case(rank, world, scheme, causal, p2p, hq, hkv, s_local, 3 if p2p else 1)
     _batch_case(rank, world, "zigzag", True, p2p, 4, 2, 640, 2, d=64)  # kD = 64 instantiations, fused and fallback
+    # fp16: the fused path's fp16 dK / dV reduction (reduce_dkv) and the fp16 delta / dq_finalize kernels
+    _batch_case(rank, world, "zigzag", True, p2p, 4, 2, 512, 2, dtype=torch.float16)
 
 
 @pytest.mark.parametrize("p2p", [True, False])
