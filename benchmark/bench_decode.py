@@ -7,9 +7,14 @@ peak), with the card name and power limit.  Under ``torchrun`` (world > 1) every
 the line also reports the all-gather + combine time of the cross-rank merge.  With ``--page-size N`` every
 configuration also times the kernel on a paged copy of the same cache (pages in a seeded random order, one block
 table per sequence) in the same alternating loop, and reports whether its output is bitwise the contiguous one.
+With ``--kv-dtype e4m3`` every configuration also times the kernel over an e4m3 copy of the cache (quantised with
+per-(sequence, kv head) descales; paged too with ``--page-size``) in the same loop, and reports its bytes, rate,
+speed-up over the bf16 kernel, whether its output at unit descales is bitwise the bf16 kernel's on the widened cache,
+and its largest difference from the bf16 output (the quantisation error, for information).
 
     python benchmark/bench_decode.py                      # B in {1, 8}, caches of 32K..512K tokens per rank
     python benchmark/bench_decode.py --page-size 16       # also the paged kernel, pages of 16 rows
+    python benchmark/bench_decode.py --kv-dtype e4m3      # also the fp8-cache kernel
     torchrun --nproc-per-node 2 benchmark/bench_decode.py
     python benchmark/bench_decode.py --dry-run            # shapes and byte counts only (no GPU)
 """
@@ -40,6 +45,8 @@ def parse_args(argv=None):
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--sm-count", type=int, default=132, help="used by --dry-run only")
     ap.add_argument("--page-size", type=int, default=None, help="also time a paged cache with pages of N rows")
+    ap.add_argument("--kv-dtype", choices=("bf16", "e4m3"), default="bf16",
+                    help="e4m3: also time an fp8 (e4m3) cache with per-head descales")
     ap.add_argument("--dry-run", action="store_true")
     return ap.parse_args(argv)
 
@@ -53,6 +60,8 @@ def shapes(args, sm_count):
                        kv_bytes=b * s * args.hkv * args.head_dim * 2 * 2)
             if args.page_size:
                 cfg.update(page_size=args.page_size, block_table_bytes=b * -(-s // args.page_size) * 4)
+            if args.kv_dtype == "e4m3":  # one byte per cached element
+                cfg.update(kv_dtype="e4m3", fp8_kv_bytes=cfg["kv_bytes"] // 2)
             yield cfg
 
 
@@ -110,21 +119,49 @@ def main():
         def ours():
             return dec.kernel_decode(q, kc, vc, sl, None, None, True, scale)
 
+        fp8 = args.kv_dtype == "e4m3"
+        fp8_res = {}
+        if fp8:  # e4m3 copies with per-(sequence, kv head) descales amax / 448, one sequence at a time
+            kd = torch.stack([kc[i].abs().amax(dim=(0, 2)).float() for i in range(b)]).clamp(min=1e-12) / 448
+            vd = torch.stack([vc[i].abs().amax(dim=(0, 2)).float() for i in range(b)]).clamp(min=1e-12) / 448
+            k8 = torch.stack([dec.quantize_e4m3(kc[i], kd[i]) for i in range(b)])
+            v8 = torch.stack([dec.quantize_e4m3(vc[i], vd[i]) for i in range(b)])
+
+            def ours_fp8():
+                return dec.kernel_decode(q, k8, v8, sl, None, None, True, scale, k_descale=kd, v_descale=vd)
+
+            ones = torch.ones_like(kd)
+            wk, wv = k8.to(torch.bfloat16), v8.to(torch.bfloat16)  # the widened cache
+            unit = dec.kernel_decode(q, k8, v8, sl, None, None, True, scale, k_descale=ones, v_descale=ones)
+            wide = dec.kernel_decode(q, wk, wv, sl, None, None, True, scale)
+            fp8_res["fp8_unit_descale_bitwise_equal_bf16"] = all(torch.equal(x, y) for x, y in zip(unit, wide))
+            del wk, wv, unit, wide
+            fp8_res["fp8_max_abs_diff_vs_bf16"] = (ours_fp8()[0].float() - ours()[0].float()).abs().max().item()
+
         if args.page_size:  # the same rows in a pool whose pages are in a seeded random order
             ps = args.page_size
             max_blocks = -(-s // ps)
             perm = torch.randperm(b * max_blocks, generator=torch.Generator().manual_seed(rank)).to(dev)
             table = perm.to(torch.int32).view(b, max_blocks)
-            pk = kc.new_zeros(b * max_blocks, ps, args.hkv, d)
-            pv = vc.new_zeros(b * max_blocks, ps, args.hkv, d)
-            for src, pool in ((kc, pk), (vc, pv)):
+
+            def to_pool(src):
+                pool = src.new_zeros(b * max_blocks, ps, args.hkv, d)
                 pad = src.new_zeros(b, max_blocks * ps, args.hkv, d)
                 pad[:, :s] = src
                 pool[perm.long()] = pad.view(b * max_blocks, ps, args.hkv, d)
-                del pad
+                return pool
+
+            pk, pv = to_pool(kc), to_pool(vc)
 
             def paged():
                 return dec.kernel_decode(q, pk, pv, sl, None, None, True, scale, block_table=table)
+
+            if fp8:
+                p8k, p8v = to_pool(k8.view(torch.uint8)).view(k8.dtype), to_pool(v8.view(torch.uint8)).view(v8.dtype)
+
+                def paged_fp8():
+                    return dec.kernel_decode(q, p8k, p8v, sl, None, None, True, scale, block_table=table,
+                                             k_descale=kd, v_descale=vd)
 
         # SDPA reads the same shard through (B, H, S, D) views
         qt, kt, vt = q.transpose(1, 2), kc.transpose(1, 2), vc.transpose(1, 2)
@@ -135,11 +172,19 @@ def main():
         rows = {"ours": [], "sdpa": []}
         if args.page_size:
             rows["paged"] = []
+        if fp8:
+            rows["fp8"] = []
+            if args.page_size:
+                rows["paged_fp8"] = []
         sdpa_err = None
         for _ in range(3):  # alternate them in one run
             rows["ours"].append(time_us(ours, args.iters, args.warmup))
             if args.page_size:
                 rows["paged"].append(time_us(paged, args.iters, args.warmup))
+            if fp8:
+                rows["fp8"].append(time_us(ours_fp8, args.iters, args.warmup))
+                if args.page_size:
+                    rows["paged_fp8"].append(time_us(paged_fp8, args.iters, args.warmup))
             if sdpa_err is None:
                 try:
                     rows["sdpa"].append(time_us(sdpa, args.iters, args.warmup))
@@ -150,14 +195,21 @@ def main():
         for k, ts in rows.items():
             if ts:
                 us = min(ts)
+                nbytes = cfg["fp8_kv_bytes"] if k.endswith("fp8") else cfg["kv_bytes"]
                 res[f"{k}_us"] = round(us, 2)
                 res[f"{k}_us_all"] = [round(t, 2) for t in ts]
-                res[f"{k}_GBps"] = round(cfg["kv_bytes"] / (us * 1e-6) / 1e9, 1)
-                res[f"{k}_share_of_datasheet_hbm"] = round(cfg["kv_bytes"] / (us * 1e-6) / HBM_DATASHEET_BPS, 3)
+                res[f"{k}_GBps"] = round(nbytes / (us * 1e-6) / 1e9, 1)
+                res[f"{k}_share_of_datasheet_hbm"] = round(nbytes / (us * 1e-6) / HBM_DATASHEET_BPS, 3)
         if sdpa_err:
             res["sdpa_error"] = sdpa_err
         if args.page_size:
             res["paged_equal_contiguous"] = all(torch.equal(x, y) for x, y in zip(paged(), ours()))
+        if fp8:
+            res["fp8_speedup_vs_bf16"] = round(res["ours_us"] / res["fp8_us"], 3)
+            if args.page_size:
+                res["paged_fp8_speedup_vs_paged"] = round(res["paged_us"] / res["paged_fp8_us"], 3)
+                res["paged_fp8_equal_contiguous_fp8"] = all(torch.equal(x, y) for x, y in zip(paged_fp8(), ours_fp8()))
+            res.update(fp8_res)
         if world > 1:
             C = dec.cuda_ext.load()
             n_out = b * args.sq * args.hq * d
@@ -177,6 +229,10 @@ def main():
         del q, kc, vc
         if args.page_size:
             del pk, pv
+        if fp8:
+            del k8, v8
+            if args.page_size:
+                del p8k, p8v
         torch.cuda.empty_cache()
     if world > 1:
         dist.destroy_process_group()

@@ -230,7 +230,9 @@ const char* lse_unflatten_launch(const float* in, float* out, const int* cu, int
 const char* make_plain_tensor_map(CUtensorMap* out, const TensorView& t, int elem_bytes, int box_rows, int dim_inner);
 
 // Encode a (rows, heads, 128) tensor as a 3-D TMA map with a (64, 1, box_rows) box and 128-byte swizzle.
-// elem_bytes is 2 (bf16/fp16) or 4 (fp32; then the box is 32 elements wide).
-const char* make_tensor_map(CUtensorMap* out, const TensorView& t, int elem_bytes, int box_rows, int dim_inner);
+// elem_bytes is 2 (bf16/fp16) or 4 (fp32; then the box is 32 elements wide) or 1 (e4m3: 128 elements).
+// swizzle_bytes 64 selects the 64-byte swizzle and a box half as wide (e4m3 rows of 64 elements).
+const char* make_tensor_map(CUtensorMap* out, const TensorView& t, int elem_bytes, int box_rows, int dim_inner,
+                            int swizzle_bytes = 128);
 
 }  // namespace rfa

@@ -401,15 +401,20 @@ at::Tensor lse_unflatten(const at::Tensor& lse, const at::Tensor& cu, int64_t ma
 // batch and sequence dimensions; seqlens (B,) int32; k_new / v_new (B, Sq, Hkv, D) contiguous, appended to the caches
 // before attention when given.  part: fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq), see DecodeParams.  With block_table
 // (B, max_blocks) int32, the caches are page pools (num_blocks, page_size, Hkv, D) with mergeable page and row
-// dimensions, and S_cap = max_blocks * page_size.
+// dimensions, and S_cap = max_blocks * page_size.  The caches may instead both be float8_e4m3fn, with k_descale /
+// v_descale fp32 (B, Hkv) contiguous on q's device: the cache then holds x / descale[b, kv head].
 void decode_fwd(const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
                 const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
-                double scale, at::Tensor& part, const c10::optional<at::Tensor>& block_table) {
+                double scale, at::Tensor& part, const c10::optional<at::Tensor>& block_table,
+                const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale) {
   const c10::cuda::CUDAGuard guard(q.device());
   TORCH_CHECK(q.dim() == 4 && k_cache.dim() == 4 && v_cache.dim() == 4, "decode_fwd: 4-D q / k_cache / v_cache");
   TORCH_CHECK(k_cache.sizes() == v_cache.sizes(), "decode_fwd: k_cache and v_cache shapes differ");
-  TORCH_CHECK(k_cache.scalar_type() == q.scalar_type() && v_cache.scalar_type() == q.scalar_type(),
-              "decode_fwd: caches must have q's dtype");
+  const bool fp8 = k_cache.scalar_type() == at::kFloat8_e4m3fn;
+  TORCH_CHECK(k_cache.scalar_type() == v_cache.scalar_type() && (fp8 || k_cache.scalar_type() == q.scalar_type()),
+              "decode_fwd: caches must both have q's dtype or both be fp8 (float8_e4m3fn)");
+  TORCH_CHECK(k_descale.has_value() == fp8 && v_descale.has_value() == fp8,
+              "decode_fwd: fp8 caches need k_descale and v_descale, and other caches take none");
   const int64_t B = q.size(0), sq = q.size(1), hq = q.size(2), d = q.size(3);
   const bool paged = block_table.has_value();
   const int64_t page_size = paged ? k_cache.size(1) : 0;
@@ -474,10 +479,18 @@ void decode_fwd(const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, c
     p.page_size = static_cast<int>(page_size);
     p.num_pages = static_cast<int>(k_cache.size(0));
   }
+  if (fp8) {
+    for (const at::Tensor* t : {&*k_descale, &*v_descale})
+      TORCH_CHECK(t->scalar_type() == at::kFloat && t->is_cuda() && t->device() == q.device() && t->dim() == 2 &&
+                      t->size(0) == B && t->size(1) == hkv && t->is_contiguous(),
+                  "decode_fwd: fp8 descales must be contiguous fp32 (B, Hkv) on q's device");
+    p.k_descale = k_descale->data_ptr<float>();
+    p.v_descale = v_descale->data_ptr<float>();
+  }
   const TensorView kv{k_cache.data_ptr(), cache_rows, static_cast<int>(hkv), k_cache.stride(1), k_cache.stride(2)};
   const TensorView vv{v_cache.data_ptr(), cache_rows, static_cast<int>(hkv), v_cache.stride(1), v_cache.stride(2)};
-  check(rfa::decode_fwd_launch(dtype_code(q), kv, vv, kn, vn, p, static_cast<int>(n_splits), static_cast<int>(d),
-                               at::cuda::getCurrentCUDAStream()));
+  check(rfa::decode_fwd_launch(dtype_code(q), fp8 ? rfa::kDtypeE4M3 : dtype_code(q), kv, vv, kn, vn, p,
+                               static_cast<int>(n_splits), static_cast<int>(d), at::cuda::getCurrentCUDAStream()));
 }
 
 // Merges the partials of decode_fwd (or gathered per-rank partials, same layout): out (B, Sq, Hq, D) contiguous in

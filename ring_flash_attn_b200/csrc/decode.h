@@ -28,13 +28,17 @@ struct DecodeParams {
   long long bt_stride;     // table entries between consecutive sequences
   int page_size;           // 0: contiguous (B, S_cap, Hkv, D) caches; else 16, 32, 64 or a multiple of 128
   int num_pages;
+  // e4m3 caches: the cache holds x / descale, per (sequence, kv head); nullptr for bf16 / fp16 caches
+  const float* k_descale;  // (B, Hkv) contiguous
+  const float* v_descale;
 };
 
-// Appends k_new / v_new (B, Sq, Hkv, D), contiguous, at rows [seqlens[b], seqlens[b] + Sq) of the caches (rows past
-// the capacity, and with a block table rows whose page id is outside the pool, are dropped), then runs the split-KV
-// kernel.  k_new == nullptr: attention only.
-const char* decode_fwd_launch(int dtype, const TensorView& k_cache, const TensorView& v_cache, const void* k_new,
-                              const void* v_new, const DecodeParams& p, int n_splits, int head_dim,
+// Appends k_new / v_new (B, Sq, Hkv, D), contiguous, in q's dtype, at rows [seqlens[b], seqlens[b] + Sq) of the
+// caches (rows past the capacity, and with a block table rows whose page id is outside the pool, are dropped), then
+// runs the split-KV kernel.  k_new == nullptr: attention only.  cache_dtype is dtype, or kDtypeE4M3 with
+// p.k_descale / p.v_descale set: the append then stores e4m3(x / descale), saturated to +-448.
+const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_cache, const TensorView& v_cache,
+                              const void* k_new, const void* v_new, const DecodeParams& p, int n_splits, int head_dim,
                               cudaStream_t stream);
 
 // Merges n_parts partials (part_stride elements apart) row by row in partial order.  out_dtype: kDtypeBF16,

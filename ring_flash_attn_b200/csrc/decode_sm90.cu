@@ -10,6 +10,12 @@
 // Roles (160 threads): warpgroup 0 computes (S = Q K^T, mask, softmax, O += P V, epilogue); warp 4 is the TMA
 // producer (one thread).
 //
+// e4m3 caches (288 threads): the producer (warp 8) TMA-loads e4m3 tiles into a ring of fp8 slots, and a converter
+// warpgroup (warps 4-7) widens each one, exactly, into the bf16 / fp16 slot layout TMA fills for a bf16 / fp16 cache,
+// then arrives on that slot's kv_full barrier.  The compute warpgroup is the same code; k_descale[b, kv head]
+// multiplies its scale_log2 once and v_descale[b, kv head] its 1 / l.  So with power-of-two descales 2^a, 2^c the
+// result is bitwise the bf16 / fp16 kernel's on the widened cache with softmax_scale * 2^a, out scaled by 2^c.
+//
 // Visibility: key j of the shard is visible to query token t iff j < seqlens[b] + n_vis(t), where n_vis(t) counts
 // the keys this call appended to this shard that t may see (0 on every rank but the append rank; t + 1 when causal,
 // Sq otherwise).  Cache rows at or past that limit are never read into a result: their K columns are masked to
@@ -28,18 +34,34 @@ namespace dec {
 constexpr int kTile = 128;    // keys per K / V tile
 constexpr int kRows = 64;     // packed query rows per CTA (one wgmma M)
 constexpr int kStages = 6;    // K/V ring slots (one key tile takes two: K, then V)
+constexpr int kStagesFp8 = 4;  // the same with an e4m3 cache, whose kF8Stages fp8 slots take the rest of the memory
+constexpr int kF8Stages = 4;
 constexpr int kThreads = 160;  // one compute warpgroup + one producer warp
+constexpr int kThreadsFp8 = 288;  // + one converter warpgroup
 constexpr int kKHalfBytes = kTile * 128;  // one 64-element-wide (128-byte) swizzled K / V sub-tile
 constexpr int kQHalfBytes = kRows * 128;  // the same for the query tile
 
-template <int kD>
+template <int kD, bool kFp8>
 constexpr int smem_bytes() {
-  return kRows * kD * 2 + kStages * kTile * kD * 2 + 1024 /*barriers*/ + 1024 /*align slack*/;
+  return kRows * kD * 2 + (kFp8 ? kStagesFp8 * kTile * kD * 3 : kStages * kTile * kD * 2) + 1024 /*barriers*/ +
+         1024 /*align slack*/;
 }
 
 struct Barriers {
   uint64_t kv_full[kStages];
   uint64_t kv_empty[kStages];
+  uint64_t f8_full[kF8Stages];  // e4m3 caches: the fp8 slots
+  uint64_t f8_empty[kF8Stages];
+};
+
+// The ring the TMA producer fills: bf16 / fp16 slots of kD / 64 128-byte-swizzled sub-tiles of 128-byte rows, or
+// e4m3 slots of one sub-tile of kD-byte rows (128-byte swizzle at kD = 128, 64-byte at kD = 64).
+template <int kD, bool kFp8>
+struct LoadRing {
+  static constexpr int kSlots = kFp8 ? kF8Stages : kStages;
+  static constexpr int kSubTiles = kFp8 ? 1 : kD / 64;
+  static constexpr int kRowBytes = kFp8 ? kD : 128;  // bytes per row of one sub-tile
+  static constexpr int kSlotBytes = kTile * kSubTiles * kRowBytes;
 };
 
 // Keys of the shard visible to token t (see the file comment), at most the capacity.
@@ -56,13 +78,16 @@ __device__ __forceinline__ int key_limit(const DecodeParams& p, int seqlen, int 
 // looked up nor loaded, and neither are pages whose id lies outside the pool (a caller error); the slot's expected
 // byte count covers only the boxes issued.  The rows left unwritten hold an older tile, and the compute warpgroup
 // already discards every row at or past kmax (K columns masked, V rows zeroed), exactly as for a contiguous cache.
-// Table entries are read 32 at a time, one per lane, a window ahead of use, and broadcast with shuffles.
-template <int kD>
-__device__ __forceinline__ void produce_paged(const CUtensorMap* tm_k, const CUtensorMap* tm_v, Barriers* bars,
-                                              uint8_t* smem_kv, const DecodeParams& p, int b, int kv_head, int j0,
-                                              int n_tiles, int kmax) {
-  constexpr int kSubTiles = kD / 64;
-  constexpr int kSlotBytes = kTile * kD * 2;
+// Table entries are read 32 at a time, one per lane, a window ahead of use, and broadcast with shuffles.  The e4m3
+// ring works the same way: a box of page_size < 128 rows is page_size * kD bytes, a multiple of 1024, so every box
+// starts on a swizzle period of the fp8 layout too.
+template <int kD, bool kFp8>
+__device__ __forceinline__ void produce_paged(const CUtensorMap* tm_k, const CUtensorMap* tm_v, uint64_t* full,
+                                              uint64_t* empty, uint8_t* smem_kv, const DecodeParams& p, int b,
+                                              int kv_head, int j0, int n_tiles, int kmax) {
+  using L = LoadRing<kD, kFp8>;
+  constexpr int kSubTiles = L::kSubTiles;
+  constexpr int kSlotBytes = L::kSlotBytes;
   const int lane = threadIdx.x & 31;
   const int ps = p.page_size;
   const int box = ps < kTile ? ps : kTile;  // rows per TMA box, as in the tensor maps
@@ -86,23 +111,23 @@ __device__ __forceinline__ void produce_paged(const CUtensorMap* tm_k, const CUt
     const bool live = lane < n_sub && key0 + lane * box < kmax && page >= 0 && page < p.num_pages;
     const int row = live ? page * ps + (key0 - pg0 * ps) : 0;
     const unsigned loads = __ballot_sync(0xffffffffu, live);
-    const uint32_t tx = __popc(loads) * box * 128 * kSubTiles;
+    const uint32_t tx = __popc(loads) * box * L::kRowBytes * kSubTiles;
     for (int kv = 0; kv < 2; ++kv) {
       uint8_t* dst = smem_kv + slot * kSlotBytes;
       if (lane == 0) {
-        mbar_wait(&bars->kv_empty[slot], phase ^ 1);
-        mbar_arrive_expect_tx(&bars->kv_full[slot], tx);
+        mbar_wait(&empty[slot], phase ^ 1);
+        mbar_arrive_expect_tx(&full[slot], tx);
       }
       for (int i = 0; i < n_sub; ++i) {
         const int r = __shfl_sync(0xffffffffu, row, i);
         if (lane == 0 && (loads >> i & 1u)) {
 #pragma unroll
           for (int h = 0; h < kSubTiles; ++h)
-            tma_load_3d(dst + h * kKHalfBytes + i * box * 128, kv == 0 ? tm_k : tm_v, &bars->kv_full[slot], 64 * h,
+            tma_load_3d(dst + h * kKHalfBytes + i * box * L::kRowBytes, kv == 0 ? tm_k : tm_v, &full[slot], 64 * h,
                         kv_head, r);
         }
       }
-      if (++slot == kStages) {
+      if (++slot == L::kSlots) {
         slot = 0;
         phase ^= 1;
       }
@@ -110,14 +135,53 @@ __device__ __forceinline__ void produce_paged(const CUtensorMap* tm_k, const CUt
   }
 }
 
+// two e4m3 (low 16 bits of x) -> two T in one word, exactly
+template <typename T>
+__device__ __forceinline__ uint32_t widen2(uint32_t x) {
+  if constexpr (std::is_same_v<T, __half>) return e4m3x2_to_f16x2(x);
+  else return e4m3x2_to_bf16x2(x);
+}
+
+// One e4m3 K / V tile as TMA wrote it (kTile rows of kD bytes; 128-byte swizzle at kD = 128, 64-byte at kD = 64)
+// -> the T tile TMA writes for a bf16 / fp16 cache (kD / 64 sub-tiles of 128-byte swizzled rows), by the 128 threads
+// of the converter warpgroup.  16 e4m3 values (one 16-byte chunk) per thread and step; the 8 threads of one 128-byte
+// store phase take chunks 0-3 of two adjacent rows, whose swizzled 16-byte positions are then all distinct.
 template <typename T, int kD>
-__global__ void __launch_bounds__(kThreads, 1)
+__device__ __forceinline__ void widen_tile(const uint8_t* src, uint8_t* dst, int ctid) {
+  constexpr int kChunks = kD / 16;  // e4m3 chunks per row
+#pragma unroll
+  for (int i = 0; i < kTile * kChunks / 128; ++i) {
+    const int idx = ctid + 128 * i;
+    const int r = kD == 128 ? ((idx >> 4) << 1) | ((idx >> 2) & 1) : idx >> 2;
+    const int c = kD == 128 ? (idx & 3) | ((idx >> 1) & 4) : idx & 3;
+    const int phys = kD == 128 ? c ^ (r & 7) : c ^ ((r >> 1) & 3);
+    const uint4 x = *reinterpret_cast<const uint4*>(src + r * kD + (phys << 4));
+    uint4 lo, hi;
+    lo.x = widen2<T>(x.x);
+    lo.y = widen2<T>(x.x >> 16);
+    lo.z = widen2<T>(x.y);
+    lo.w = widen2<T>(x.y >> 16);
+    hi.x = widen2<T>(x.z);
+    hi.y = widen2<T>(x.z >> 16);
+    hi.z = widen2<T>(x.w);
+    hi.w = widen2<T>(x.w >> 16);
+    uint8_t* row = dst + (c >> 2) * kKHalfBytes + r * 128;
+    const int c0 = 2 * (c & 3);
+    *reinterpret_cast<uint4*>(row + ((c0 ^ (r & 7)) << 4)) = lo;
+    *reinterpret_cast<uint4*>(row + (((c0 + 1) ^ (r & 7)) << 4)) = hi;
+  }
+}
+
+template <typename T, int kD, bool kFp8>
+__global__ void __launch_bounds__(kFp8 ? kThreadsFp8 : kThreads, 1)
 decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
               const __grid_constant__ DecodeParams p) {
   static_assert(kD == 64 || kD == 128, "head dim 64 or 128");
+  using L = LoadRing<kD, kFp8>;
   constexpr int kSubTiles = kD / 64;
+  constexpr int kSlots = kFp8 ? kStagesFp8 : kStages;  // T slots the compute warpgroup reads
   constexpr int kSlotBytes = kTile * kD * 2;
-  constexpr uint32_t kTxBytes = kSlotBytes;
+  constexpr int kProducer = kFp8 ? 256 : 128;  // first thread of the producer warp
   const int split = blockIdx.x;
   const int b = blockIdx.z / p.hkv, kv_head = blockIdx.z % p.hkv;
   const int group = p.hq / p.hkv;
@@ -137,35 +201,47 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_q = smem;
   uint8_t* smem_kv = smem + kRows * kD * 2;
-  Barriers* bars = reinterpret_cast<Barriers*>(smem_kv + kStages * kSlotBytes);
+  uint8_t* smem_f8 = smem_kv + kSlots * kSlotBytes;  // e4m3 caches only
+  Barriers* bars = reinterpret_cast<Barriers*>(smem_f8 + (kFp8 ? L::kSlots * L::kSlotBytes : 0));
+  // the ring TMA fills
+  uint8_t* smem_load = kFp8 ? smem_f8 : smem_kv;
+  uint64_t* load_full = kFp8 ? bars->f8_full : bars->kv_full;
+  uint64_t* load_empty = kFp8 ? bars->f8_empty : bars->kv_empty;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_k);
     tma_prefetch_desc(&tm_v);
-    for (int i = 0; i < kStages; ++i) {
-      mbar_init(&bars->kv_full[i], 1);
+    for (int i = 0; i < kSlots; ++i) {
+      mbar_init(&bars->kv_full[i], kFp8 ? 4 : 1);  // TMA, or one arrival per converter warp
       mbar_init(&bars->kv_empty[i], 4);  // one arrival per compute warp
+    }
+    if constexpr (kFp8) {
+      for (int i = 0; i < kF8Stages; ++i) {
+        mbar_init(&bars->f8_full[i], 1);
+        mbar_init(&bars->f8_empty[i], 4);  // one arrival per converter warp
+      }
     }
     fence_mbar_init();
   }
   __syncthreads();
 
-  if (threadIdx.x >= 128) {
+  if (threadIdx.x >= kProducer) {
     // ------------------------------------------------------------------ TMA producer
     if (p.page_size != 0) {
-      if (n_tiles > 0) produce_paged<kD>(&tm_k, &tm_v, bars, smem_kv, p, b, kv_head, j0, n_tiles, kmax);
-    } else if (threadIdx.x == 128) {
+      if (n_tiles > 0)
+        produce_paged<kD, kFp8>(&tm_k, &tm_v, load_full, load_empty, smem_load, p, b, kv_head, j0, n_tiles, kmax);
+    } else if (threadIdx.x == kProducer) {
       uint32_t slot = 0, phase = 0;
       for (int jj = 0; jj < n_tiles; ++jj) {
         const int row = b * p.s_cap + (j0 + jj) * kTile;  // rows past the tensor's end arrive as zeros
         for (int kv = 0; kv < 2; ++kv) {
-          mbar_wait(&bars->kv_empty[slot], phase ^ 1);
-          uint8_t* dst = smem_kv + slot * kSlotBytes;
-          mbar_arrive_expect_tx(&bars->kv_full[slot], kTxBytes);
+          mbar_wait(&load_empty[slot], phase ^ 1);
+          uint8_t* dst = smem_load + slot * L::kSlotBytes;
+          mbar_arrive_expect_tx(&load_full[slot], L::kSlotBytes);
 #pragma unroll
-          for (int h = 0; h < kSubTiles; ++h)
-            tma_load_3d(dst + h * kKHalfBytes, kv == 0 ? &tm_k : &tm_v, &bars->kv_full[slot], 64 * h, kv_head, row);
-          if (++slot == kStages) {
+          for (int h = 0; h < L::kSubTiles; ++h)
+            tma_load_3d(dst + h * kKHalfBytes, kv == 0 ? &tm_k : &tm_v, &load_full[slot], 64 * h, kv_head, row);
+          if (++slot == L::kSlots) {
             slot = 0;
             phase ^= 1;
           }
@@ -173,6 +249,33 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
       }
     }
     return;
+  }
+
+  if constexpr (kFp8) {
+    if (threadIdx.x >= 128) {
+      // ---------------------------------------------------------------- converter: fp8 slot -> T slot
+      uint32_t slot = 0, phase = 0, fslot = 0, fphase = 0;
+      for (int i = 0; i < 2 * n_tiles; ++i) {  // K, V, K, V, ...
+        mbar_wait(&bars->f8_full[fslot], fphase);
+        mbar_wait(&bars->kv_empty[slot], phase ^ 1);
+        widen_tile<T, kD>(smem_f8 + fslot * L::kSlotBytes, smem_kv + slot * kSlotBytes, threadIdx.x - 128);
+        fence_proxy_async_smem();  // the generic-proxy writes, before wgmma reads them
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) {
+          mbar_arrive(&bars->kv_full[slot]);
+          mbar_arrive(&bars->f8_empty[fslot]);
+        }
+        if (++slot == kSlots) {
+          slot = 0;
+          phase ^= 1;
+        }
+        if (++fslot == kF8Stages) {
+          fslot = 0;
+          fphase ^= 1;
+        }
+      }
+      return;
+    }
   }
 
   // -------------------------------------------------------------------- compute warpgroup
@@ -211,7 +314,8 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
   float m2[2] = {-CUDART_INF_F, -CUDART_INF_F};
   float l[2] = {0.f, 0.f};
-  const float t2 = p.scale_log2;
+  float t2 = p.scale_log2;
+  if constexpr (kFp8) t2 *= p.k_descale[b * p.hkv + kv_head];
 
   const uint64_t q_desc = gmma_desc(smem_u32(smem_q), 0);         // K-major A
   const uint64_t k_desc0 = gmma_desc(smem_u32(smem_kv), 0);       // K tile, K-major B
@@ -220,12 +324,12 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   uint32_t slot = 0, phase = 0;
   for (int jj = 0; jj < n_tiles; ++jj) {
     const uint32_t k_slot = slot, k_phase = phase;
-    if (++slot == kStages) {
+    if (++slot == kSlots) {
       slot = 0;
       phase ^= 1;
     }
     const uint32_t v_slot = slot, v_phase = phase;
-    if (++slot == kStages) {
+    if (++slot == kSlots) {
       slot = 0;
       phase ^= 1;
     }
@@ -332,7 +436,8 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
     if (r >= rows_here) continue;
     const int pr = row0 + r;
     const int t = pr / group, head = kv_head * group + pr % group;
-    const float inv = lt > 0.f ? 1.0f / lt : 0.f;
+    float inv = lt > 0.f ? 1.0f / lt : 0.f;
+    if constexpr (kFp8) inv *= p.v_descale[b * p.hkv + kv_head];
     float* out_row = part + ((static_cast<long long>(b) * p.sq + t) * p.hq + head) * kD;
 #pragma unroll
     for (int j = 0; j < kD / 8; ++j)
@@ -345,6 +450,17 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   }
 }
 
+// Cache row of new key t of sequence b (the pool row with a block table), or -1 when the row is dropped: past the
+// capacity, or with a page id outside the pool.
+__device__ __forceinline__ long long append_row(const DecodeParams& p, int b, int t) {
+  const int row = p.seqlens[b] + t;
+  if (row < 0 || row >= p.s_cap) return -1;
+  if (p.page_size == 0) return static_cast<long long>(b) * p.s_cap + row;
+  const int page = p.block_table[b * p.bt_stride + row / p.page_size];
+  if (page < 0 || page >= p.num_pages) return -1;
+  return static_cast<long long>(page) * p.page_size + row % p.page_size;
+}
+
 // One block per (b, t) row of the new keys, blockIdx.y selects K or V.  16-byte chunks; rows past the capacity
 // are dropped, and so are rows whose page id lies outside the pool.
 __global__ void decode_append_kernel(uint8_t* k_cache, uint8_t* v_cache, long long row_stride_bytes,
@@ -352,14 +468,8 @@ __global__ void decode_append_kernel(uint8_t* k_cache, uint8_t* v_cache, long lo
                                      const DecodeParams p, int row_bytes) {
   const int sq = p.sq, hkv = p.hkv;
   const int b = blockIdx.x / sq, t = blockIdx.x % sq;
-  const int row = p.seqlens[b] + t;
-  if (row < 0 || row >= p.s_cap) return;
-  long long cache_row = static_cast<long long>(b) * p.s_cap + row;
-  if (p.page_size != 0) {
-    const int page = p.block_table[b * p.bt_stride + row / p.page_size];
-    if (page < 0 || page >= p.num_pages) return;
-    cache_row = static_cast<long long>(page) * p.page_size + row % p.page_size;
-  }
+  const long long cache_row = append_row(p, b, t);
+  if (cache_row < 0) return;
   uint8_t* dst = (blockIdx.y == 0 ? k_cache : v_cache) + cache_row * row_stride_bytes;
   const uint8_t* src = (blockIdx.y == 0 ? k_new : v_new) + static_cast<long long>(blockIdx.x) * hkv * row_bytes;
   const int chunks = row_bytes / 16;
@@ -367,6 +477,33 @@ __global__ void decode_append_kernel(uint8_t* k_cache, uint8_t* v_cache, long lo
     const int head = idx / chunks, c = idx % chunks;
     *reinterpret_cast<uint4*>(dst + head * head_stride_bytes + 16 * c) =
         *reinterpret_cast<const uint4*>(src + static_cast<long long>(head) * row_bytes + 16 * c);
+  }
+}
+
+// The same into e4m3 caches: x / descale[b, head] (IEEE division), saturated to +-448 and rounded to nearest even
+// (NaN stays NaN), 8 values per step.
+template <typename T>
+__global__ void decode_append_e4m3_kernel(uint8_t* k_cache, uint8_t* v_cache, long long row_stride,
+                                          long long head_stride, const T* k_new, const T* v_new,
+                                          const DecodeParams p, int head_dim) {
+  const int sq = p.sq, hkv = p.hkv;
+  const int b = blockIdx.x / sq, t = blockIdx.x % sq;
+  const long long cache_row = append_row(p, b, t);
+  if (cache_row < 0) return;
+  uint8_t* dst = (blockIdx.y == 0 ? k_cache : v_cache) + cache_row * row_stride;
+  const T* src = (blockIdx.y == 0 ? k_new : v_new) + static_cast<long long>(blockIdx.x) * hkv * head_dim;
+  const float* descale = (blockIdx.y == 0 ? p.k_descale : p.v_descale) + b * hkv;
+  const int chunks = head_dim / 8;
+  for (int idx = threadIdx.x; idx < hkv * chunks; idx += blockDim.x) {
+    const int head = idx / chunks, c = idx % chunks;
+    const float ds = descale[head];
+    const uint4 raw = *reinterpret_cast<const uint4*>(src + static_cast<long long>(head) * head_dim + 8 * c);
+    const T* x = reinterpret_cast<const T*>(&raw);
+    float f[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) f[j] = __fdiv_rn(static_cast<float>(x[j]), ds);
+    *reinterpret_cast<uint2*>(dst + head * head_stride + 8 * c) =
+        make_uint2(pack4_e4m3(f[0], f[1], f[2], f[3]), pack4_e4m3(f[4], f[5], f[6], f[7]));
   }
 }
 
@@ -414,11 +551,15 @@ __global__ void decode_combine_kernel(const float* parts, long long part_stride,
 
 }  // namespace dec
 
-const char* decode_fwd_launch(int dtype, const TensorView& k_cache, const TensorView& v_cache, const void* k_new,
-                              const void* v_new, const DecodeParams& p, int n_splits, int head_dim,
+const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_cache, const TensorView& v_cache,
+                              const void* k_new, const void* v_new, const DecodeParams& p, int n_splits, int head_dim,
                               cudaStream_t stream) {
   if (head_dim != 64 && head_dim != 128) return "the sm_90a decode kernel is instantiated for head_dim 64 and 128";
   if (dtype != kDtypeBF16 && dtype != kDtypeFP16) return "the sm_90a decode kernel takes bf16 / fp16";
+  const bool fp8 = cache_dtype == kDtypeE4M3;
+  if (!fp8 && cache_dtype != dtype) return "the caches must have q's dtype or be e4m3";
+  if (fp8 != (p.k_descale != nullptr && p.v_descale != nullptr))
+    return "e4m3 caches need k / v descales, and only e4m3 caches take them";
   if (p.hkv <= 0 || p.hq % p.hkv != 0) return "query heads must be a multiple of kv heads";
   if (k_cache.row_stride != v_cache.row_stride || k_cache.head_stride != v_cache.head_stride)
     return "k_cache and v_cache must have the same strides";
@@ -430,28 +571,49 @@ const char* decode_fwd_launch(int dtype, const TensorView& k_cache, const Tensor
   }
   // a paged cache's tensor maps cover the whole pool; a box is at most one page
   const int box_rows = p.page_size != 0 && p.page_size < dec::kTile ? p.page_size : dec::kTile;
+  // e4m3 rows are head_dim bytes: one 128-byte swizzle span at head_dim 128, one 64-byte span at 64
+  const int elem_bytes = fp8 ? 1 : 2;
+  const int swizzle = fp8 ? head_dim : 128;
   CUtensorMap tk, tv;
-  if (const char* e = make_tensor_map(&tk, k_cache, 2, box_rows, head_dim)) return e;
-  if (const char* e = make_tensor_map(&tv, v_cache, 2, box_rows, head_dim)) return e;
+  if (const char* e = make_tensor_map(&tk, k_cache, elem_bytes, box_rows, head_dim, swizzle)) return e;
+  if (const char* e = make_tensor_map(&tv, v_cache, elem_bytes, box_rows, head_dim, swizzle)) return e;
   if (k_new != nullptr && p.n_new > 0) {
-    dec::decode_append_kernel<<<dim3(p.batch * p.sq, 2), 128, 0, stream>>>(
-        static_cast<uint8_t*>(k_cache.ptr), static_cast<uint8_t*>(v_cache.ptr), k_cache.row_stride * 2,
-        k_cache.head_stride * 2, static_cast<const uint8_t*>(k_new), static_cast<const uint8_t*>(v_new), p,
-        head_dim * 2);
+    const dim3 agrid(p.batch * p.sq, 2);
+    uint8_t* kc = static_cast<uint8_t*>(k_cache.ptr);
+    uint8_t* vc = static_cast<uint8_t*>(v_cache.ptr);
+    if (!fp8)
+      dec::decode_append_kernel<<<agrid, 128, 0, stream>>>(kc, vc, k_cache.row_stride * 2, k_cache.head_stride * 2,
+                                                           static_cast<const uint8_t*>(k_new),
+                                                           static_cast<const uint8_t*>(v_new), p, head_dim * 2);
+    else if (dtype == kDtypeBF16)
+      dec::decode_append_e4m3_kernel<<<agrid, 128, 0, stream>>>(
+          kc, vc, k_cache.row_stride, k_cache.head_stride, static_cast<const __nv_bfloat16*>(k_new),
+          static_cast<const __nv_bfloat16*>(v_new), p, head_dim);
+    else
+      dec::decode_append_e4m3_kernel<<<agrid, 128, 0, stream>>>(kc, vc, k_cache.row_stride, k_cache.head_stride,
+                                                                static_cast<const __half*>(k_new),
+                                                                static_cast<const __half*>(v_new), p, head_dim);
   }
   const int row_tiles = (p.sq * (p.hq / p.hkv) + dec::kRows - 1) / dec::kRows;
-  dim3 grid(n_splits, row_tiles, p.batch * p.hkv), block(dec::kThreads, 1, 1);
+  const dim3 grid(n_splits, row_tiles, p.batch * p.hkv);
   cudaError_t err = cudaSuccess;
-  auto launch = [&](auto kern, int smem) {
+  auto launch = [&](auto kern, int smem, int threads) {
     err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (err == cudaSuccess) kern<<<grid, block, smem, stream>>>(tk, tv, p);
+    if (err == cudaSuccess) kern<<<grid, threads, smem, stream>>>(tk, tv, p);
+  };
+  auto pick = [&](auto t, auto f8) {
+    using T = decltype(t);
+    constexpr bool kFp8 = decltype(f8)::value;
+    const int threads = kFp8 ? dec::kThreadsFp8 : dec::kThreads;
+    if (head_dim == 128) launch(dec::decode_kernel<T, 128, kFp8>, dec::smem_bytes<128, kFp8>(), threads);
+    else launch(dec::decode_kernel<T, 64, kFp8>, dec::smem_bytes<64, kFp8>(), threads);
   };
   if (dtype == kDtypeBF16) {
-    if (head_dim == 128) launch(dec::decode_kernel<__nv_bfloat16, 128>, dec::smem_bytes<128>());
-    else launch(dec::decode_kernel<__nv_bfloat16, 64>, dec::smem_bytes<64>());
+    if (fp8) pick(__nv_bfloat16{}, std::true_type{});
+    else pick(__nv_bfloat16{}, std::false_type{});
   } else {
-    if (head_dim == 128) launch(dec::decode_kernel<__half, 128>, dec::smem_bytes<128>());
-    else launch(dec::decode_kernel<__half, 64>, dec::smem_bytes<64>());
+    if (fp8) pick(__half{}, std::true_type{});
+    else pick(__half{}, std::false_type{});
   }
   if (err != cudaSuccess) return cudaGetErrorString(err);
   err = cudaGetLastError();

@@ -270,6 +270,16 @@ __device__ __forceinline__ uint32_t e4m3x2_to_bf16x2(uint32_t x) {
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(f.y), "f"(f.x));
   return r;
 }
+// two e4m3 (low 16 bits of x) -> two fp16 in one 32-bit word (exact: every e4m3 value is an fp16 value)
+__device__ __forceinline__ uint32_t e4m3x2_to_f16x2(uint32_t x) {
+  uint32_t h;
+  asm("{\n\t.reg .b16 lo;\n\t"
+      "cvt.u16.u32 lo, %1;\n\t"
+      "cvt.rn.f16x2.e4m3x2 %0, lo;\n\t}\n"
+      : "=r"(h)
+      : "r"(x));
+  return h;
+}
 
 // ------------------------------------------------------------------ misc
 __device__ __forceinline__ float fast_exp2(float x) {

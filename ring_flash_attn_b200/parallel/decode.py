@@ -86,10 +86,12 @@ def _capacity(k_cache: Tensor, block_table: Optional[Tensor]) -> int:
 
 def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor, k: Optional[Tensor],
                   v: Optional[Tensor], causal: bool, softmax_scale: float, pg=None, world: int = 1,
-                  splits: Optional[int] = None, block_table: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+                  splits: Optional[int] = None, block_table: Optional[Tensor] = None,
+                  k_descale: Optional[Tensor] = None, v_descale: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
     """Local split-KV kernel (appending ``k`` / ``v`` first when given), then the combine over the splits and, for
     ``world > 1``, over the gathered per-rank partials.  ``splits`` overrides :func:`num_splits`.  With
-    ``block_table`` the caches are page pools (see :func:`cp_flash_attn_with_kvcache`)."""
+    ``block_table`` the caches are page pools (see :func:`cp_flash_attn_with_kvcache`).  e4m3 caches take contiguous
+    fp32 ``(B, Hkv)`` ``k_descale`` / ``v_descale``."""
     C = cuda_ext.load()
     b, sq, hq, d = q.shape
     q = q.contiguous()
@@ -101,7 +103,8 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
     n_out = b * sq * hq * d
     size = n_out + b * hq * sq
     parts = torch.empty((splits, size), dtype=torch.float32, device=q.device)
-    C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts, block_table)
+    C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts, block_table, k_descale,
+                 v_descale)
     cuda_ext.note_launch(2 if k is not None else 1)
     if world > 1:
         mine = torch.empty(size, dtype=torch.float32, device=q.device)
@@ -119,14 +122,25 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
 # dense path
 # ----------------------------------------------------------------------------------------------
 
-def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table=None):
+def quantize_e4m3(x: Tensor, descale: Tensor) -> Tensor:
+    """``x`` (..., Hkv, D) as stored in an e4m3 cache with per-kv-head ``descale`` (Hkv,): IEEE division, saturation
+    to +-448, then round-to-nearest-even (NaN stays NaN)."""
+    return (x.float() / descale[:, None]).clamp(-448, 448).to(torch.float8_e4m3fn)
+
+
+def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table=None,
+                  k_descale=None, v_descale=None):
     b, sq, hq, d = q.shape
     s_cap = _capacity(k_cache, block_table)
     lens = [max(0, min(int(x), s_cap)) for x in cache_seqlens.tolist()]
     n_new = sq if k is not None else 0
     ps, n_pages = k_cache.shape[1], k_cache.shape[0]
     table = block_table.tolist() if block_table is not None else None
+    fp8 = k_descale is not None
     if k is not None:  # rows past the capacity (or whose page is outside the pool) are dropped, as in the kernel path
+        if fp8:
+            k = torch.stack([quantize_e4m3(k[i], k_descale[i]) for i in range(b)])
+            v = torch.stack([quantize_e4m3(v[i], v_descale[i]) for i in range(b)])
         for i, n in enumerate(lens):
             m = min(sq, s_cap - n)
             if table is None:
@@ -151,6 +165,8 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
             if not all(0 <= x < n_pages for x in pages):
                 raise ValueError(f"block_table[{i}] points outside the {n_pages}-page pool for a page it reads")
             kk, vv = k_cache[pages].flatten(0, 1)[:n_keys], v_cache[pages].flatten(0, 1)[:n_keys]
+        if fp8:  # the dequantised rows
+            kk, vv = kk.float() * k_descale[i][:, None], vv.float() * v_descale[i][:, None]
         # appended key u (row n + u) is visible to token t iff u <= t, i.e. row j <= t + n
         diag = n if (n_new and causal) else None
         out[i], lse[i] = block_fwd(q[i], kk, vv, softmax_scale, diag)
@@ -174,10 +190,12 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
 @torch.library.custom_op("rfa_b200::cp_decode", mutates_args=("k_cache", "v_cache"))
 def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor, k: Optional[Tensor],
               v: Optional[Tensor], append_rank: int, softmax_scale: float, causal: bool, group: str,
-              block_table: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
+              block_table: Optional[Tensor], k_descale: Optional[Tensor],
+              v_descale: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
     """q (B, Sq, Hq, D) -> (out (B, Sq, Hq, D) in q.dtype, lse (B, Hq, Sq) fp32).  ``k`` / ``v`` are appended to
     the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's name ("" = world);
-    with ``block_table`` the caches are this rank's page pools."""
+    with ``block_table`` the caches are this rank's page pools; e4m3 caches come with contiguous fp32 (B, Hkv)
+    ``k_descale`` / ``v_descale``."""
     pg = resolve_group(group)
     rank, world = group_info(pg)
     if k is not None and not 0 <= append_rank < world:
@@ -186,12 +204,14 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
         k = v = None
     if _kernel_takes(q):
         return kernel_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world,
-                             block_table=block_table)
-    return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table)
+                             block_table=block_table, k_descale=k_descale, v_descale=v_descale)
+    return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table,
+                         k_descale, v_descale)
 
 
 @cp_decode.register_fake
-def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group, block_table):
+def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group, block_table, k_descale,
+      v_descale):
     b, sq, hq, _ = q.shape
     return q.new_empty(q.shape), q.new_empty((b, hq, sq), dtype=torch.float32)
 
@@ -217,9 +237,23 @@ def _check_block_table(q, k_cache, v_cache, block_table):
         raise ValueError("num_blocks * page_size and max_blocks * page_size must be below 2^31")
 
 
+def _check_descale(name, x, q, b, hkv):
+    """An fp8 cache's descale as the contiguous (B, Hkv) fp32 tensor the kernels read."""
+    if x is None:
+        raise ValueError(f"fp8 caches need {name} (fp32, shape (), (Hkv,) or (B, Hkv))")
+    if not isinstance(x, Tensor) or x.dtype != torch.float32:
+        raise ValueError(f"fp8 {name} must be a float32 tensor")
+    if x.device != q.device:
+        raise ValueError(f"fp8 {name} must be on q's device")
+    if tuple(x.shape) not in ((), (hkv,), (b, hkv)):
+        raise ValueError(f"fp8 {name} must have shape (), (Hkv,) or (B, Hkv) = {(b, hkv)}, not {tuple(x.shape)}")
+    return x.expand(b, hkv).contiguous()
+
+
 def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=None, append_rank=None,
                                softmax_scale=None, causal=True, return_softmax_lse=False, group=None, *,
-                               block_table=None, window_size=(-1, -1), alibi_slopes=None):
+                               block_table=None, k_descale=None, v_descale=None, window_size=(-1, -1),
+                               alibi_slopes=None):
     """Decode attention of new query tokens against a KV cache sharded over ``group`` (modelled on flash-attn's
     ``flash_attn_with_kvcache``).  Inference only: no gradient.
 
@@ -236,6 +270,15 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
       On the append rank the caller allocates the pages of rows ``[0, cache_seqlens[b] + Sq)`` before the call.
       An entry outside the pool for a page that is read is a caller error: the kernel's result is then undefined,
       but it never accesses memory outside the pool (the dense path raises ``ValueError``).
+    * fp8 caches: ``k_cache`` / ``v_cache`` may both be ``torch.float8_e4m3fn`` (contiguous or paged), with a bf16 /
+      fp16 ``q``.  ``k_descale`` / ``v_descale`` are then required: fp32 tensors on q's device of shape ``()``,
+      ``(Hkv,)`` or ``(B, Hkv)``, and the cache stands for ``k_cache.float() * k_descale[b, h]`` (the same for V).
+      Each rank passes the descales of its own shard; ranks may differ.  They are read on the device only (a CUDA
+      graph replay uses their current contents) and are not validated: non-finite or non-positive descales give an
+      undefined result.  The appended ``k`` / ``v`` stay in q's dtype and are stored as
+      ``(x.float() / descale).clamp(-448, 448).to(torch.float8_e4m3fn)``.  An e4m3 cache holds twice the tokens of
+      a bf16 one and a decode step reads half the bytes.  Descales given with a bf16 / fp16 cache, fp8 queries,
+      ``float8_e5m2`` caches, mixed cache dtypes and fp8 caches with an fp32 ``q`` raise ``ValueError``.
     * ``cache_seqlens`` ``(B,)`` int32 on q's device: valid rows of this rank's shard (0 = empty shard).
     * ``k`` / ``v`` ``(B, Sq, Hkv, D)``, optional, the same on every rank: written in place into the caches of rank
       ``append_rank`` only, at rows ``[cache_seqlens[b], cache_seqlens[b] + Sq)``, before attention (rows past
@@ -245,9 +288,9 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
       ``0..t`` of its own call (flash-attn's bottom-right alignment); with ``causal=False`` all ``Sq`` of them.
     * Returns ``out`` ``(B, Sq, Hq, D)`` in q.dtype, and ``softmax_lse`` ``(B, Hq, Sq)`` fp32 when
       ``return_softmax_lse``.  Both are bitwise identical on every rank.
-    * ``window_size``, ``alibi_slopes``, fp8 caches, ``D > 128`` and ``Hq % Hkv != 0`` raise ``ValueError``.  The
-      sm_90a kernel covers bf16 / fp16 with ``D`` in {64, 128}; other head sizes run the dense torch path with a
-      one-time warning.
+    * ``window_size``, ``alibi_slopes``, ``D > 128`` and ``Hq % Hkv != 0`` raise ``ValueError``.  The sm_90a kernel
+      covers a bf16 / fp16 ``q`` with ``D`` in {64, 128}, over caches in q's dtype or e4m3; other head sizes run the
+      dense torch path with a one-time warning.
     * Nothing is read back to the host on the kernel path, so a decode step can be captured in a CUDA graph.
 
     RoPE: the positions of the new tokens are the caller's to apply (prefill length plus the decode step)."""
@@ -261,10 +304,23 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
     hkv = k_cache.shape[2]
     if (block_table is None and k_cache.shape[0] != b) or k_cache.shape[3] != d or sq < 1:
         raise ValueError(f"q {tuple(q.shape)} does not match the cache {tuple(k_cache.shape)}")
-    if q.element_size() == 1 or k_cache.element_size() == 1 or v_cache.element_size() == 1:
-        raise ValueError("cp_flash_attn_with_kvcache: fp8 queries / caches are not supported")
-    if k_cache.dtype != q.dtype or v_cache.dtype != q.dtype:
-        raise ValueError("k_cache / v_cache must have q's dtype")
+    if q.element_size() == 1:
+        raise ValueError("cp_flash_attn_with_kvcache: fp8 queries are not supported")
+    if k_cache.element_size() == 1 or v_cache.element_size() == 1:
+        if k_cache.dtype != v_cache.dtype:
+            raise ValueError(f"fp8 caches: k_cache ({k_cache.dtype}) and v_cache ({v_cache.dtype}) must both be "
+                             "torch.float8_e4m3fn")
+        if k_cache.dtype != torch.float8_e4m3fn:
+            raise ValueError(f"fp8 caches must be torch.float8_e4m3fn, not {k_cache.dtype}")
+        if q.dtype not in (torch.bfloat16, torch.float16):
+            raise ValueError(f"fp8 caches need a bf16 / fp16 q, not {q.dtype}")
+        k_descale = _check_descale("k_descale", k_descale, q, b, hkv)
+        v_descale = _check_descale("v_descale", v_descale, q, b, hkv)
+    else:
+        if k_cache.dtype != q.dtype or v_cache.dtype != q.dtype:
+            raise ValueError("k_cache / v_cache must have q's dtype")
+        if k_descale is not None or v_descale is not None:
+            raise ValueError("k_descale / v_descale are only taken with fp8 (float8_e4m3fn) caches")
     if d > 128:
         raise ValueError(f"cp_flash_attn_with_kvcache: head_dim {d} > 128 is not supported")
     if hq % hkv != 0:
@@ -286,5 +342,5 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
         raise ValueError("append_rank must be None when no k / v are given")
     scale = float(softmax_scale) if softmax_scale is not None else d ** -0.5
     out, lse = cp_decode(q, k_cache, v_cache, cache_seqlens, k, v, -1 if append_rank is None else int(append_rank),
-                         scale, bool(causal), group_name(group), block_table)
+                         scale, bool(causal), group_name(group), block_table, k_descale, v_descale)
     return (out, lse) if return_softmax_lse else out
