@@ -24,10 +24,10 @@ torch.cuda.synchronize()
 C.set_trace(None)
 t = trace.cpu().view(64, 16)
 base = int(t[t > 0].min())
-names = ["mma:top", "mma:dSok", "mma:dPiss", "mma:dqfree", "mma:dQiss", "mma:end", "sm:Sfull", "sm:Parr", "sm:dPfull",
-         "sm:dSarr", "-", "dr:dqfull", "dr:done"]
-print("tile " + " ".join(f"{n:>10s}" for n in names))
+# slots written by thread 0 of CTA 0 per query tile (attn_bwd_sm90.cu, RFA_STAMP)
+names = ["S^T ready", "dP^T ready", "dS^T staged", "dQ issued"]
+print("tile " + " ".join(f"{n:>12s}" for n in names))
 for i in range(6, 26):
-    print(f"{i:4d} " + " ".join(f"{(int(x) - base) if x > 0 else -1:10d}" for x in t[i][:13]))
+    print(f"{i:4d} " + " ".join(f"{(int(x) - base) if x > 0 else -1:12d}" for x in t[i][:len(names)]))
 per = [(int(t[i + 1][0]) - int(t[i][0])) for i in range(8, 40) if t[i + 1][0] > 0 and t[i][0] > 0]
-print("cycles per tile (mma:top deltas):", per[:16], "mean", sum(per) / max(1, len(per)))
+print("cycles per tile (S^T ready deltas):", per[:16], "mean", sum(per) / max(1, len(per)))

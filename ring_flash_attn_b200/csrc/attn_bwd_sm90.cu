@@ -17,6 +17,11 @@
 //                            read MN-major; B = K MN-major) -> fp32 shared memory -> TMA reduce-add
 // Both warpgroups meet at three named barriers per query tile (dS^T complete, dQ staged, previous tile retired),
 // so the Q / dO ring needs no "empty" barriers: thread 0 refills the stage of tile i - 1 while tile i runs.
+// Each stage also holds the 64 lse and delta values of its rows and a description of its tile.  Threads 0-63 copy
+// lse / delta for tile i + 2 (one row each, coalesced, cp.async: no register held in flight) at the top of tile i
+// and wait for the copies before its first barrier, so the softmax reads shared memory and no global load sits
+// between a GEMM's completion and the exp2 that needs it.  S^T and dP^T are separate commit groups: P^T is
+// computed while dP^T still runs.
 #include <math_constants.h>
 #include <stdio.h>
 
@@ -28,7 +33,7 @@ namespace rfa {
 namespace bwd {
 
 #ifdef RFA_TRACE
-// per-tile stamps of CTA 0 (16 slots), thread 0: 0 S^T / dP^T complete, 1 dS^T staged, 2 dQ issued
+// per-tile stamps of CTA 0 (16 slots), thread 0: 0 S^T complete, 1 dP^T complete, 2 dS^T staged, 3 dQ issued
 #define RFA_STAMP(cond, iter, slot)                                                              \
   do {                                                                                            \
     if ((cond) && cta == 0 && p.trace != nullptr && (iter) < 64) p.trace[(iter)*16 + (slot)] = clock64(); \
@@ -52,14 +57,21 @@ struct Geo {
   static constexpr int kKVBytes = kTileK * kD * 2;  // K, V tile: 32 KB at kD = 128
   static constexpr int kQBytes = kTileQ * kD * 2;   // Q, dO tile: 16 KB
   static constexpr int kDQBytes = kTileQ * kD * 4;  // fp32 dQ staging: 32 KB
-  static constexpr int kSmemBytes =
-      2 * kKVBytes + kStages * 2 * kQBytes + kDSBytes + kDQBytes + 1024 /*barriers*/ + 1024 /*slack*/;
+  static constexpr int kSmemBytes = 2 * kKVBytes + kStages * 2 * kQBytes + kDSBytes + kDQBytes +
+                                    kStages * 2 * kTileQ * 4 /*lse2, delta*/ + 1024 /*barriers*/ + 1024 /*slack*/;
 };
 
 struct Barriers {
   uint64_t kv_full;
   uint64_t qdo_full[kStages];
 };
+// The query tile in a Q/dO stage, as the consumers need it (written by the loader with the stage; the consumers keep
+// no tile iterator of their own in registers)
+struct alignas(16) StageTile {
+  int ti, diag, lo;
+  int head, row;  // of the tile's dQ rows (first row)
+};
+static_assert(sizeof(Barriers) + kStages * sizeof(StageTile) <= 1024, "barrier area");
 
 // Query tiles of one segment that can see this key tile.
 struct QGeom {
@@ -143,7 +155,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   uint8_t* smem_qdo = smem_v + kKVBytes;                 // kStages x (Q 16 KB, dO 16 KB)
   uint8_t* smem_ds = smem_qdo + kStages * 2 * kQBytes;   // 16 KB, [128 keys][64 queries] swizzled
   float* smem_dq = reinterpret_cast<float*>(smem_ds + kDSBytes);   // [64 queries][kD dims] fp32
-  Barriers* bars = reinterpret_cast<Barriers*>(reinterpret_cast<uint8_t*>(smem_dq) + kDQBytes);
+  // [kStages][64] lse (natural log, as the forward wrote it), then [kStages][64] delta; 32-bit shared addresses
+  constexpr uint32_t kLseBytes = kStages * kTileQ * 4;
+  const uint32_t lse_base = smem_u32(smem_dq) + kDQBytes;
+  Barriers* bars = reinterpret_cast<Barriers*>(reinterpret_cast<uint8_t*>(smem_dq) + kDQBytes + 2 * kLseBytes);
+  StageTile* tiles = reinterpret_cast<StageTile*>(bars + 1);  // [kStages]
 
   const int tid = threadIdx.x;
   const int lane = tid & 31;
@@ -167,26 +183,46 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   }
   const int total_tiles = tiles_per_head * group;
 
-  // ---------------------------------------------------------------- loads (thread 0)
+  // ---------------------------------------------------------------- loads (threads 0-63; TMA: thread 0)
   // (a tile no local query reaches only sends zero rows: nothing is loaded, and in particular no TMA write can
   // land in the K | V area after the epilogue has started to stage those rows there)
   TileIter ld;
   ld.init(p.qsegs, it.seg_begin, it.seg_count, group);
   int n_loaded = 0;
   auto load_next = [&]() {
-    const int stage = n_loaded % kStages;
-    const int head = kv_head * group + ld.gq;
-    const int row = ld.g.q_row0 + ld.ti * kTileQ;
-    uint8_t* dq_ = smem_qdo + stage * 2 * kQBytes;
-    uint8_t* ddo = dq_ + kQBytes;
-    mbar_arrive_expect_tx(&bars->qdo_full[stage], 2 * kQBytes);
+    if (tid == 0) {
+      const int stage = n_loaded % kStages;
+      const int head = kv_head * group + ld.gq;
+      const int row = ld.g.q_row0 + ld.ti * kTileQ;
+      uint8_t* dq_ = smem_qdo + stage * 2 * kQBytes;
+      uint8_t* ddo = dq_ + kQBytes;
+      mbar_arrive_expect_tx(&bars->qdo_full[stage], 2 * kQBytes);
 #pragma unroll
-    for (int h = 0; h < kSubTiles; ++h) {
-      tma_load_3d(dq_ + h * kQHalf, &tm_q, &bars->qdo_full[stage], 64 * h, head, row);
-      tma_load_3d(ddo + h * kQHalf, &tm_do, &bars->qdo_full[stage], 64 * h, head, row);
+      for (int h = 0; h < kSubTiles; ++h) {
+        tma_load_3d(dq_ + h * kQHalf, &tm_q, &bars->qdo_full[stage], 64 * h, head, row);
+        tma_load_3d(ddo + h * kQHalf, &tm_do, &bars->qdo_full[stage], 64 * h, head, row);
+      }
+      // (its slot was last read by tile n_loaded - kStages, which every thread finished before barrier 1)
+      tiles[stage] = StageTile{ld.ti, ld.g.diag, ld.g.lo, head, row};
     }
     ++n_loaded;
     ld.next();
+  };
+  // lse and delta of row `tid` of the tile being loaded -> the stage's slots, with cp.async (no register is held
+  // while the copy is in flight; complete after cp_async_wait_all).  Rows that do not exist: lse -inf, delta 0.
+  auto lse_stage = [&]() {
+    const uint32_t sl = lse_base + ((n_loaded % kStages) * kTileQ + tid) * 4;
+    const int qi = ld.ti * kTileQ + tid;
+    if (qi < ld.g.q_len) {
+      const int row = ld.g.q_row0 + qi;
+      const size_t b = row / p.lse_S, sidx = row % p.lse_S;
+      const size_t idx = (b * p.hq + kv_head * group + ld.gq) * static_cast<size_t>(p.lse_S) + sidx;
+      cp_async_4(sl, p.lse + idx);
+      cp_async_4(sl + kLseBytes, p.delta + idx);
+    } else {
+      st_shared_f32(sl, -CUDART_INF_F);
+      st_shared_f32(sl + kLseBytes, 0.f);
+    }
   };
   if (tid == 0) {
     tma_prefetch_desc(&tm_q);
@@ -213,8 +249,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         tma_load_3d(smem_k + h * kKVHalf, mk, &bars->kv_full, 64 * h, kv_head, it.kv_row0);
         tma_load_3d(smem_v + h * kKVHalf, mv, &bars->kv_full, 64 * h, kv_head, it.kv_row0);
       }
-      while (n_loaded < kStages - 1 && n_loaded < total_tiles) load_next();
     }
+  }
+  if (tid < kTileQ) {
+    while (n_loaded < kStages - 1 && n_loaded < total_tiles) {
+      lse_stage();
+      load_next();
+    }
+    cp_async_wait_all();
   }
   __syncthreads();
 
@@ -234,17 +276,17 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const uint64_t k_mn = gmma_desc(k_base + w * kKVHalf, kKVHalf);     // K[:, 64 w : 64 w + 64], MN-major B
 
   if (total_tiles > 0) mbar_wait(&bars->kv_full, 0);
-  TileIter cur;
-  cur.init(p.qsegs, it.seg_begin, it.seg_count, group);
-  for (int i = 0; i < total_tiles; ++i, cur.next()) {
+  for (int i = 0; i < total_tiles; ++i) {
     const int stage = i % kStages;
-    const int head = kv_head * group + cur.gq;
-    const QGeom& g = cur.g;
-    const int ti = cur.ti;
+    const StageTile g = tiles[stage];
+    const int ti = g.ti;
+    // lse / delta of tile i + 2 into the slot of tile i - 1 (whose softmax every thread finished before the
+    // barriers of tile i - 1): copied under this tile's GEMMs and softmax, complete before barrier 1
+    if (tid < kTileQ && n_loaded < total_tiles) lse_stage();
     mbar_wait(&bars->qdo_full[stage], (i / kStages) & 1);
     const uint32_t st_off = stage * 2 * kQBytes;
 
-    // ---- S^T, dP^T
+    // ---- S^T, dP^T (two commit groups)
     float st[32], dpt[32];
     wgmma_fence();
 #pragma unroll
@@ -253,6 +295,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       const uint32_t ob = st_off + (k >> 2) * kQHalf + (k & 3) * 32;
       Gmma<T>::template ss64<0, 0>(st, gmma_desc_add(k_km, oa), gmma_desc_add(q_km0, ob), k > 0);
     }
+    wgmma_commit();
 #pragma unroll
     for (int k = 0; k < kD / 16; ++k) {
       const uint32_t oa = (k >> 2) * kKVHalf + (k & 3) * 32;
@@ -275,34 +318,43 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         q_hi[h] = last_q < 0 ? 0 : (last_q >= kTileQ ? kTileQ : static_cast<int>(last_q) + 1);
       }
     }
-    wgmma_wait<0>();
+    wgmma_wait<1>();
     fence_regs(st);
-    fence_regs(dpt);
     RFA_STAMP(tid == 0, i, 0);
 
-    // ---- P^T (into st), dS^T (into dpt).  lse in log2 units: +inf for rows that do not exist or saw no key => P = 0
+    // ---- P^T (into st) while dP^T runs.  lse in log2 units: +inf for rows that do not exist or saw no key => P = 0
+    const uint32_t lse = lse_base + stage * kTileQ * 4;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int c = 8 * j + quad_col + e;
-        const int qi = ti * kTileQ + c;
-        float lse2 = CUDART_INF_F, dl = 0.f;
-        if (qi < g.q_len) {
-          const int row = g.q_row0 + qi;
-          const size_t b = row / p.lse_S, sidx = row % p.lse_S;
-          const size_t idx = (b * p.hq + head) * static_cast<size_t>(p.lse_S) + sidx;
-          const float x = p.lse[idx];
-          lse2 = x == -CUDART_INF_F ? CUDART_INF_F : x * 1.4426950408889634f;
-          dl = p.delta[idx];
-        }
+        const float x = ld_shared_f32(lse + c * 4);
+        const float l = x == -CUDART_INF_F ? CUDART_INF_F : x * 1.4426950408889634f;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int r = 4 * j + 2 * h + e;
-          const float pe = fast_exp2(fmaf(st[r], p.scale_log2, -lse2));
-          const float pv = (c >= q_lo[h] && c < q_hi[h]) ? pe : 0.f;
-          st[r] = pv;
-          dpt[r] = pv * (dpt[r] - dl) * p.scale;
+          const float pe = fast_exp2(fmaf(st[r], p.scale_log2, -l));
+          st[r] = (c >= q_lo[h] && c < q_hi[h]) ? pe : 0.f;
+        }
+      }
+    }
+    wgmma_wait<0>();
+    fence_regs(dpt);
+    RFA_STAMP(tid == 0, i, 1);
+
+    // ---- dS^T (into dpt)
+    const uint32_t delta = lse_base + kLseBytes + stage * kTileQ * 4;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int c = 8 * j + quad_col + e;
+        const float dl = ld_shared_f32(delta + c * 4);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = 4 * j + 2 * h + e;
+          dpt[r] = st[r] * (dpt[r] - dl) * p.scale;
         }
       }
     }
@@ -324,9 +376,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
     // tile i - 1 has retired everywhere past this barrier: its dQ has been read out of smem_dq by the reduce, the
     // dQ GEMMs no longer read smem_ds, and its Q / dO stage may be refilled
+    if (tid < kTileQ) cp_async_wait_all();
     if (tid == 0) tma_store_wait_read<0>();
     named_bar_sync(1, kThreads);
-    if (tid == 0 && n_loaded < total_tiles) load_next();
+    if (tid < kTileQ && n_loaded < total_tiles) load_next();
 
     // ---- dS^T -> shared memory: [128 keys][64 queries] bf16, 128-byte swizzled rows
 #pragma unroll
@@ -340,7 +393,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     }
     fence_proxy_async_smem();
     named_bar_sync(2, kThreads);
-    RFA_STAMP(tid == 0, i, 1);
+    RFA_STAMP(tid == 0, i, 2);
 
     // ---- dQ[:, 64 w : 64 w + 64] = dS K[:, 64 w : 64 w + 64]   (head dim 64: group 0 computes all of dQ)
     float dq[32];
@@ -369,10 +422,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     fence_proxy_async_smem();
     named_bar_sync(3, kThreads);
     if (tid == 0) {
-      tma_reduce_add_3d(&tm_dq, smem_dq, 0, head, g.q_row0 + ti * kTileQ);
+      tma_reduce_add_3d(&tm_dq, smem_dq, 0, tiles[stage].head, tiles[stage].row);
       tma_store_commit();
     }
-    RFA_STAMP(tid == 0, i, 2);
+    RFA_STAMP(tid == 0, i, 3);
   }
   if (tid == 0) tma_store_wait<0>();
 

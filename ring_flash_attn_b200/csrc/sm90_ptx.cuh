@@ -73,6 +73,23 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
+// ------------------------------------------------------------------ cp.async (Ampere-style, per thread)
+// 4-byte global -> shared copy that holds no register while in flight; visible to the issuing thread after
+// cp_async_wait_all, to the others after a barrier that follows it.
+__device__ __forceinline__ void cp_async_4(uint32_t saddr, const void* gsrc) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(saddr), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+// shared-window accesses by 32-bit address (no generic 64-bit pointer to keep in registers)
+__device__ __forceinline__ float ld_shared_f32(uint32_t saddr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(saddr));
+  return v;
+}
+__device__ __forceinline__ void st_shared_f32(uint32_t saddr, float v) {
+  asm volatile("st.shared.f32 [%0], %1;" ::"r"(saddr), "f"(v) : "memory");
+}
+
 // ------------------------------------------------------------------ TMA (tiled, 3-D tensor maps)
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
