@@ -14,7 +14,8 @@
 //   dV_w += P^T dO_i         (A = P^T from registers, B = dO MN-major)
 //   dK_w += dS^T Q_i         (A = dS^T from registers, B = Q MN-major)
 //   dQ_i[:, 64 w : 64 w + 64] = dS_i K[:, 64 w : 64 w + 64]   (A = dS^T of both groups in shared memory,
-//                            read MN-major; B = K MN-major) -> fp32 shared memory -> TMA reduce-add
+//                            read MN-major; B = K MN-major) -> fp32 shared memory (128-byte swizzled boxes of
+//                            32 dims) -> TMA reduce-add
 // Both warpgroups meet at three named barriers per query tile (dS^T complete, dQ staged, previous tile retired),
 // so the Q / dO ring needs no "empty" barriers: thread 0 refills the stage of tile i - 1 while tile i runs.
 // Each stage also holds the 64 lse and delta values of its rows and a description of its tile.  Threads 0-63 copy
@@ -33,7 +34,8 @@ namespace rfa {
 namespace bwd {
 
 #ifdef RFA_TRACE
-// per-tile stamps of CTA 0 (16 slots), thread 0: 0 S^T complete, 1 dP^T complete, 2 dS^T staged, 3 dQ issued
+// per-tile stamps of CTA 0 (16 slots), thread 0: 0 S^T complete, 1 dP^T complete, 2 dS^T staged, 3 dQ issued,
+// 4 dQ complete, 5 dQ reduce-add issued, 6 S^T issued, 7 dV / dK issued (benchmark/trace_bwd.py)
 #define RFA_STAMP(cond, iter, slot)                                                              \
   do {                                                                                            \
     if ((cond) && cta == 0 && p.trace != nullptr && (iter) < 64) p.trace[(iter)*16 + (slot)] = clock64(); \
@@ -296,6 +298,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       Gmma<T>::template ss64<0, 0>(st, gmma_desc_add(k_km, oa), gmma_desc_add(q_km0, ob), k > 0);
     }
     wgmma_commit();
+    RFA_STAMP(tid == 0, i, 6);
 #pragma unroll
     for (int k = 0; k < kD / 16; ++k) {
       const uint32_t oa = (k >> 2) * kKVHalf + (k & 3) * 32;
@@ -373,6 +376,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) gmma_rs<T, kD>(dk, da[kk], gmma_desc_add(q_mn0, st_off + kk * 2048), 1);
     wgmma_commit();
+    RFA_STAMP(tid == 0, i, 7);
 
     // tile i - 1 has retired everywhere past this barrier: its dQ has been read out of smem_dq by the reduce, the
     // dQ GEMMs no longer read smem_ds, and its Q / dO stage may be refilled
@@ -405,27 +409,39 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         Gmma<T>::template ss64<1, 1>(dq, gmma_desc_add(ds_mn, k * 2048), gmma_desc_add(k_mn, k * 2048), k > 0);
       wgmma_commit();
     }
+    RFA_STAMP(tid == 0, i, 3);
     wgmma_wait<0>();
     fence_regs(dv);
     fence_regs(dk);
+    RFA_STAMP(tid == 0, i, 4);
     if (do_dq) {
       fence_regs(dq);
+      // smem_dq holds the tile as kD / 32 boxes of [64 queries][32 dims] fp32, 128-byte rows with the TMA 128-byte
+      // swizzle (16-byte unit u of row q at u ^ (q & 7)), so that the eight rows one store instruction writes fall
+      // into distinct banks: 2 shared-memory wavefronts per warp store instead of 8 with 512-byte unswizzled rows
       const int q0 = 16 * (wtid >> 5) + (lane >> 2);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        float* dst = smem_dq + (q0 + 8 * h) * kD + 64 * w + quad_col;
+        const int q = q0 + 8 * h;
+        uint8_t* row = reinterpret_cast<uint8_t*>(smem_dq) + q * 128 + (quad_col & 3) * 4;
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
-          *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(dq[4 * j + 2 * h], dq[4 * j + 2 * h + 1]);
+        for (int j = 0; j < 8; ++j) {
+          const int box = 2 * w + (j >> 2), unit = 2 * (j & 3) + (quad_col >> 2);
+          *reinterpret_cast<float2*>(row + box * (kTileQ * 128) + ((unit ^ (q & 7)) << 4)) =
+              make_float2(dq[4 * j + 2 * h], dq[4 * j + 2 * h + 1]);
+        }
       }
     }
     fence_proxy_async_smem();
     named_bar_sync(3, kThreads);
     if (tid == 0) {
-      tma_reduce_add_3d(&tm_dq, smem_dq, 0, tiles[stage].head, tiles[stage].row);
+#pragma unroll
+      for (int b = 0; b < kD / 32; ++b)
+        tma_reduce_add_3d(&tm_dq, reinterpret_cast<uint8_t*>(smem_dq) + b * (kTileQ * 128), 32 * b, tiles[stage].head,
+                          tiles[stage].row);
       tma_store_commit();
     }
-    RFA_STAMP(tid == 0, i, 3);
+    RFA_STAMP(tid == 0, i, 5);
   }
   if (tid == 0) tma_store_wait<0>();
 
@@ -563,7 +579,7 @@ const char* attn_bwd_launch(int dtype, const TensorView& q, const TensorView& do
   if (const char* e = make_tensor_map(&tv, v, 2, bwd::kTileK, d)) return e;
   if (const char* e = make_tensor_map(&tks, k_stage, 2, bwd::kTileK, d)) return e;
   if (const char* e = make_tensor_map(&tvs, v_stage, 2, bwd::kTileK, d)) return e;
-  if (const char* e = make_plain_tensor_map(&tdq, dq_accum, 4, bwd::kTileQ, d)) return e;
+  if (const char* e = make_tensor_map(&tdq, dq_accum, 4, bwd::kTileQ, d)) return e;  // 32-float swizzled boxes
   dim3 grid(n_blocks, 1, 1), block(bwd::kThreads, 1, 1);
   cudaError_t err;
   err = cudaSuccess;
