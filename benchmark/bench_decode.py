@@ -11,10 +11,15 @@ With ``--kv-dtype e4m3`` every configuration also times the kernel over an e4m3 
 per-(sequence, kv head) descales; paged too with ``--page-size``) in the same loop, and reports its bytes, rate,
 speed-up over the bf16 kernel, whether its output at unit descales is bitwise the bf16 kernel's on the widened cache,
 and its largest difference from the bf16 output (the quantisation error, for information).
+With ``--mixed-chunk C`` every configuration also times, in the same loop, a varlen call (``cu_seqlens_q``) where
+sequence 0 brings C new tokens and the others 1, the uniform call padded to Sq = C (what a caller without varlen
+must do) and the uniform Sq = 1 call (the pure-decode floor), with the K + V bytes the varlen and padded calls stream
+(every 64-row tile streams its sequence's shard).
 
     python benchmark/bench_decode.py                      # B in {1, 8}, caches of 32K..512K tokens per rank
     python benchmark/bench_decode.py --page-size 16       # also the paged kernel, pages of 16 rows
     python benchmark/bench_decode.py --kv-dtype e4m3      # also the fp8-cache kernel
+    python benchmark/bench_decode.py --mixed-chunk 64     # also a ragged batch: one 64-token chunk + decodes
     torchrun --nproc-per-node 2 benchmark/bench_decode.py
     python benchmark/bench_decode.py --dry-run            # shapes and byte counts only (no GPU)
 """
@@ -47,6 +52,9 @@ def parse_args(argv=None):
     ap.add_argument("--page-size", type=int, default=None, help="also time a paged cache with pages of N rows")
     ap.add_argument("--kv-dtype", choices=("bf16", "e4m3"), default="bf16",
                     help="e4m3: also time an fp8 (e4m3) cache with per-head descales")
+    ap.add_argument("--mixed-chunk", type=int, default=None, metavar="C",
+                    help="also time a varlen batch (sequence 0 brings C tokens, the others 1) against the uniform "
+                         "call padded to Sq = C and the uniform Sq = 1 call")
     ap.add_argument("--dry-run", action="store_true")
     return ap.parse_args(argv)
 
@@ -62,6 +70,17 @@ def shapes(args, sm_count):
                 cfg.update(page_size=args.page_size, block_table_bytes=b * -(-s // args.page_size) * 4)
             if args.kv_dtype == "e4m3":  # one byte per cached element
                 cfg.update(kv_dtype="e4m3", fp8_kv_bytes=cfg["kv_bytes"] // 2)
+            if args.mixed_chunk:
+                c, g = args.mixed_chunk, args.hq // args.hkv
+                total_q = c + b - 1
+                shard = s * args.hkv * args.head_dim * 2 * 2  # one sequence's K + V
+                chunk_tiles = -(-c * g // dec.ROWS_PER_CTA)
+                # every 64-row tile streams its sequence's shard: the bytes the varlen and padded calls move
+                cfg.update(mixed_chunk=c, varlen_total_q=total_q,
+                           tile_slots=dec.tile_slots(b, total_q, c, args.hq, args.hkv),
+                           varlen_splits=dec.num_splits_varlen(b, total_q, c, args.hq, args.hkv, s, sm_count),
+                           padded_splits=dec.num_splits(b, c, args.hq, args.hkv, s, sm_count),
+                           varlen_kv_bytes=(chunk_tiles + b - 1) * shard, padded_kv_bytes=b * chunk_tiles * shard)
             yield cfg
 
 
@@ -163,6 +182,23 @@ def main():
                     return dec.kernel_decode(q, p8k, p8v, sl, None, None, True, scale, block_table=table,
                                              k_descale=kd, v_descale=vd)
 
+        if args.mixed_chunk:  # sequence 0 brings C new tokens, the others 1, over the same caches
+            c = args.mixed_chunk
+            q_pad = torch.randn(b, c, args.hq, d, device=dev, dtype=torch.bfloat16)
+            counts = [c] + [1] * (b - 1)
+            q_var = torch.cat([q_pad[i, :n] for i, n in enumerate(counts)])
+            cu = torch.tensor([0] + [c + i for i in range(b)], dtype=torch.int32, device=dev)
+            q_one = q_pad[:, :1].contiguous()
+
+            def mixed():
+                return dec.kernel_decode(q_var, kc, vc, sl, None, None, True, scale, cu_seqlens_q=cu, max_seqlen_q=c)
+
+            def padded():
+                return dec.kernel_decode(q_pad, kc, vc, sl, None, None, True, scale)
+
+            def decode_only():
+                return dec.kernel_decode(q_one, kc, vc, sl, None, None, True, scale)
+
         # SDPA reads the same shard through (B, H, S, D) views
         qt, kt, vt = q.transpose(1, 2), kc.transpose(1, 2), vc.transpose(1, 2)
 
@@ -176,9 +212,14 @@ def main():
             rows["fp8"] = []
             if args.page_size:
                 rows["paged_fp8"] = []
+        mixed_rows = {"mixed_varlen": [], "mixed_padded": [], "mixed_decode_only": []}
         sdpa_err = None
         for _ in range(3):  # alternate them in one run
             rows["ours"].append(time_us(ours, args.iters, args.warmup))
+            if args.mixed_chunk:
+                mixed_rows["mixed_varlen"].append(time_us(mixed, args.iters, args.warmup))
+                mixed_rows["mixed_padded"].append(time_us(padded, args.iters, args.warmup))
+                mixed_rows["mixed_decode_only"].append(time_us(decode_only, args.iters, args.warmup))
             if args.page_size:
                 rows["paged"].append(time_us(paged, args.iters, args.warmup))
             if fp8:
@@ -202,6 +243,15 @@ def main():
                 res[f"{k}_share_of_datasheet_hbm"] = round(nbytes / (us * 1e-6) / HBM_DATASHEET_BPS, 3)
         if sdpa_err:
             res["sdpa_error"] = sdpa_err
+        if args.mixed_chunk:
+            for k, ts in mixed_rows.items():
+                res[f"{k}_us"] = round(min(ts), 2)
+                res[f"{k}_us_all"] = [round(t, 2) for t in ts]
+            res["mixed_speedup_vs_padded"] = round(res["mixed_padded_us"] / res["mixed_varlen_us"], 3)
+            # the chunk's rows of the varlen call, bitwise the padded call's (sequence 0 has C tokens in both)
+            v_out, p_out = mixed()[0], padded()[0]
+            res["mixed_chunk_rows_equal_padded"] = torch.equal(v_out[:c], p_out[0]) if \
+                cfg["varlen_splits"] == cfg["padded_splits"] else None
         if args.page_size:
             res["paged_equal_contiguous"] = all(torch.equal(x, y) for x, y in zip(paged(), ours()))
         if fp8:
@@ -227,6 +277,8 @@ def main():
         if rank == 0:
             print(json.dumps(res), flush=True)
         del q, kc, vc
+        if args.mixed_chunk:
+            del q_pad, q_var, q_one
         if args.page_size:
             del pk, pv
         if fp8:

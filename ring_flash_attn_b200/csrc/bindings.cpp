@@ -402,27 +402,46 @@ at::Tensor lse_unflatten(const at::Tensor& lse, const at::Tensor& cu, int64_t ma
 // before attention when given.  part: fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq), see DecodeParams.  With block_table
 // (B, max_blocks) int32, the caches are page pools (num_blocks, page_size, Hkv, D) with mergeable page and row
 // dimensions, and S_cap = max_blocks * page_size.  The caches may instead both be float8_e4m3fn, with k_descale /
-// v_descale fp32 (B, Hkv) contiguous on q's device: the cache then holds x / descale[b, kv head].
-void decode_fwd(const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
+// v_descale fp32 (B, Hkv) contiguous on q's device: the cache then holds x / descale[b, kv head].  With cu_seqlens_q
+// (B + 1,) int32 (B = seqlens.numel()), q is varlen (total_q, Hq, D), k_new / v_new (total_q, Hkv, D), part fp32
+// (n_splits, total_q*Hq*D + Hq*total_q), and max_seqlen_q >= 1 bounds every count; cu_seqlens_q is not validated.
+void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
                 const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
                 double scale, at::Tensor& part, const c10::optional<at::Tensor>& block_table,
-                const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale) {
-  const c10::cuda::CUDAGuard guard(q.device());
-  TORCH_CHECK(q.dim() == 4 && k_cache.dim() == 4 && v_cache.dim() == 4, "decode_fwd: 4-D q / k_cache / v_cache");
+                const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale,
+                const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q) {
+  const c10::cuda::CUDAGuard guard(q_in.device());
+  const bool varlen = cu_seqlens_q.has_value();
+  TORCH_CHECK(q_in.dim() == (varlen ? 3 : 4), "decode_fwd: q must be (B, Sq, Hq, D), or (total_q, Hq, D) with "
+              "cu_seqlens_q");
+  const int64_t total_q = varlen ? q_in.size(0) : 0;
+  if (varlen) {
+    const at::Tensor& cu = *cu_seqlens_q;
+    TORCH_CHECK(cu.scalar_type() == at::kInt && cu.device() == q_in.device() && cu.is_contiguous() && cu.dim() == 1 &&
+                    cu.numel() == seqlens.numel() + 1,
+                "decode_fwd: cu_seqlens_q must be (B + 1,) int32 contiguous on q's device");
+    TORCH_CHECK(max_seqlen_q >= 1, "decode_fwd: max_seqlen_q must be >= 1");
+  }
+  // the kernel's uniform view (B, Sq): varlen q as (1, total_q) for the shape checks below
+  const at::Tensor q = varlen ? q_in.unsqueeze(0) : q_in;
+  TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4, "decode_fwd: 4-D k_cache / v_cache");
   TORCH_CHECK(k_cache.sizes() == v_cache.sizes(), "decode_fwd: k_cache and v_cache shapes differ");
   const bool fp8 = k_cache.scalar_type() == at::kFloat8_e4m3fn;
   TORCH_CHECK(k_cache.scalar_type() == v_cache.scalar_type() && (fp8 || k_cache.scalar_type() == q.scalar_type()),
               "decode_fwd: caches must both have q's dtype or both be fp8 (float8_e4m3fn)");
   TORCH_CHECK(k_descale.has_value() == fp8 && v_descale.has_value() == fp8,
               "decode_fwd: fp8 caches need k_descale and v_descale, and other caches take none");
-  const int64_t B = q.size(0), sq = q.size(1), hq = q.size(2), d = q.size(3);
+  const int64_t B = varlen ? seqlens.numel() : q.size(0);
+  const int64_t sq = varlen ? max_seqlen_q : q.size(1), hq = q.size(2), d = q.size(3);
+  const int64_t rows = varlen ? total_q : B * sq;  // packed query rows
   const bool paged = block_table.has_value();
   const int64_t page_size = paged ? k_cache.size(1) : 0;
   const int64_t s_cap = paged ? block_table->size(1) * page_size : k_cache.size(1);
   const int64_t hkv = k_cache.size(2);
   const int64_t cache_rows = k_cache.size(0) * k_cache.size(1);
   TORCH_CHECK((paged || k_cache.size(0) == B) && k_cache.size(3) == d, "decode_fwd: cache shape does not match q");
-  TORCH_CHECK(q.stride(3) == 1 && q.stride(0) == sq * q.stride(1), "decode_fwd: q must be (B, Sq) mergeable");
+  TORCH_CHECK(q.stride(3) == 1 && (varlen || q.stride(0) == sq * q.stride(1)),
+              "decode_fwd: q must be (B, Sq) mergeable");
   TORCH_CHECK((q.stride(1) * 2) % 16 == 0 && (q.stride(2) * 2) % 16 == 0 &&
                   reinterpret_cast<uintptr_t>(q.data_ptr()) % 16 == 0,
               "decode_fwd: q rows must be 16-byte aligned");
@@ -442,16 +461,20 @@ void decode_fwd(const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, c
   TORCH_CHECK(seqlens.scalar_type() == at::kInt && seqlens.is_cuda() && seqlens.is_contiguous() && seqlens.numel() == B,
               "decode_fwd: cache_seqlens must be (B,) int32 on the device");
   TORCH_CHECK(part.scalar_type() == at::kFloat && part.is_contiguous() && part.dim() == 2 && part.size(0) >= 1 &&
-                  part.size(1) == B * sq * hq * d + B * hq * sq,
-              "decode_fwd: part must be fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq)");
+                  part.size(1) == rows * hq * d + rows * hq,
+              "decode_fwd: part must be fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq), or total_q for B*Sq when varlen");
   TORCH_CHECK(k_new.has_value() == v_new.has_value(), "decode_fwd: pass both k_new and v_new or neither");
   const void* kn = nullptr;
   const void* vn = nullptr;
   if (k_new.has_value()) {
-    for (const at::Tensor* t : {&*k_new, &*v_new})
-      TORCH_CHECK(t->is_contiguous() && t->scalar_type() == q.scalar_type() && t->dim() == 4 && t->size(0) == B &&
-                      t->size(1) == sq && t->size(2) == hkv && t->size(3) == d,
-                  "decode_fwd: k_new / v_new must be contiguous (B, Sq, Hkv, D) in q's dtype");
+    for (const at::Tensor* t : {&*k_new, &*v_new}) {
+      const bool shape_ok = varlen ? t->dim() == 3 && t->size(0) == total_q && t->size(1) == hkv && t->size(2) == d
+                                   : t->dim() == 4 && t->size(0) == B && t->size(1) == sq && t->size(2) == hkv &&
+                                         t->size(3) == d;
+      TORCH_CHECK(t->is_contiguous() && t->scalar_type() == q.scalar_type() && shape_ok,
+                  "decode_fwd: k_new / v_new must be contiguous (B, Sq, Hkv, D), or varlen (total_q, Hkv, D), in "
+                  "q's dtype");
+    }
     kn = k_new->data_ptr();
     vn = v_new->data_ptr();
   }
@@ -468,6 +491,8 @@ void decode_fwd(const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, c
   p.sq = static_cast<int>(sq);
   p.hq = static_cast<int>(hq);
   p.hkv = static_cast<int>(hkv);
+  p.cu_seqlens_q = varlen ? cu_seqlens_q->data_ptr<int>() : nullptr;
+  p.total_q = static_cast<int>(rows);
   p.s_cap = static_cast<int>(s_cap);
   p.tiles_per_split = static_cast<int>((tiles + n_splits - 1) / n_splits);
   p.n_new = kn != nullptr ? static_cast<int>(sq) : 0;

@@ -8,18 +8,24 @@
 namespace rfa {
 
 // Partial results live in one fp32 buffer per split (or per rank): the (b, t, h) rows of `out` (rows x head_dim),
-// followed by `lse` in the (b, h, t) order of the public softmax_lse.  part_stride = elements per split.
+// followed by `lse` in the (b, h, t) order of the public softmax_lse.  part_stride = elements per split.  A varlen
+// call (cu_seqlens_q set) uses the same layout at batch 1, sq = total_q: out rows (cu[b] + t, h), lse (h, cu[b] + t).
 struct DecodeParams {
-  const void* q;           // (B * Sq, Hq, D) view of (B, Sq, Hq, D)
+  const void* q;           // (B * Sq, Hq, D) view of (B, Sq, Hq, D), or varlen (total_q, Hq, D)
   long long q_row_stride;  // elements between consecutive (b, t)
   long long q_head_stride;
   const int* seqlens;      // (B,) valid cached rows of this rank's shard
   float* part;             // (n_splits, part_stride)
   long long part_stride;
-  int batch, sq, hq, hkv;
+  int batch, sq, hq, hkv;  // varlen: sq = max_seqlen_q, which bounds every count
+  // Varlen queries: sequence b owns packed rows [cu[b], cu[b + 1]) of q, k_new / v_new and out; nullptr: every
+  // sequence has sq rows, at b * sq.  Never validated: the kernels clamp every offset to [0, total_q] and every count
+  // to [0, sq], so malformed values give an undefined result but no access outside the buffers.
+  const int* cu_seqlens_q;  // (B + 1,)
+  int total_q;              // rows of q: B * sq when uniform
   int s_cap;               // cache rows per sequence
   int tiles_per_split;     // 128-key tiles of one sequence handled by one split
-  int n_new;               // keys appended to this shard by this call (0 on every rank but the append rank)
+  int n_new;               // nonzero iff keys are appended to this shard by this call (0 on all but the append rank)
   int causal;              // appended key u is visible to query token t only if u <= t
   float scale_log2;        // softmax scale * log2(e)
   // Paged caches: logical row j of sequence b is row j % page_size of page block_table[b * bt_stride + j / page_size]
@@ -36,10 +42,16 @@ struct DecodeParams {
 // Appends k_new / v_new (B, Sq, Hkv, D), contiguous, in q's dtype, at rows [seqlens[b], seqlens[b] + Sq) of the
 // caches (rows past the capacity, and with a block table rows whose page id is outside the pool, are dropped), then
 // runs the split-KV kernel.  k_new == nullptr: attention only.  cache_dtype is dtype, or kDtypeE4M3 with
-// p.k_descale / p.v_descale set: the append then stores e4m3(x / descale), saturated to +-448.
+// p.k_descale / p.v_descale set: the append then stores e4m3(x / descale), saturated to +-448.  Varlen: k_new / v_new
+// are (total_q, Hkv, D) and sequence b's n_b rows go to [seqlens[b], seqlens[b] + n_b); the grid is
+// (n_splits, decode_tile_slots(p), Hkv), each slot mapped to a (sequence, row tile) on the device.
 const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_cache, const TensorView& v_cache,
                               const void* k_new, const void* v_new, const DecodeParams& p, int n_splits, int head_dim,
                               cudaStream_t stream);
+
+// Varlen row-tile slots, from shapes only: min(B * ceil(sq * G / 64), (total_q * G + 63 * B) / 64), an upper bound
+// on sum_b ceil(n_b * G / 64) for any counts n_b <= sq that sum to total_q.
+long long decode_tile_slots(const DecodeParams& p);
 
 // Merges n_parts partials (part_stride elements apart) row by row in partial order.  out_dtype: kDtypeBF16,
 // kDtypeFP16, or -1 for fp32.

@@ -16,10 +16,16 @@
 // multiplies its scale_log2 once and v_descale[b, kv head] its 1 / l.  So with power-of-two descales 2^a, 2^c the
 // result is bitwise the bf16 / fp16 kernel's on the widened cache with softmax_scale * 2^a, out scaled by 2^c.
 //
+// Varlen queries (cu_seqlens_q): sequence b brings n_b = cu[b + 1] - cu[b] tokens.  The grid is (split, tile slot,
+// kv head) instead, with decode_tile_slots() slots, a bound from shapes on sum_b ceil(n_b * G / 64); each CTA finds
+// its (sequence, row tile) by a warp-wide prefix sum over cu, and slots past the last real tile exit at once.
+// Everything after that mapping is the uniform code with the sequence's own row base and count.
+//
 // Visibility: key j of the shard is visible to query token t iff j < seqlens[b] + n_vis(t), where n_vis(t) counts
 // the keys this call appended to this shard that t may see (0 on every rank but the append rank; t + 1 when causal,
-// Sq otherwise).  Cache rows at or past that limit are never read into a result: their K columns are masked to
-// -inf and their V rows are zeroed in shared memory before P V (the cache may hold anything there, NaN included).
+// the sequence's token count otherwise).  Cache rows at or past that limit are never read into a result: their K
+// columns are masked to -inf and their V rows are zeroed in shared memory before P V (the cache may hold anything
+// there, NaN included).
 #include <math_constants.h>
 
 #include <type_traits>
@@ -64,11 +70,53 @@ struct LoadRing {
   static constexpr int kSlotBytes = kTile * kSubTiles * kRowBytes;
 };
 
-// Keys of the shard visible to token t (see the file comment), at most the capacity.
-__device__ __forceinline__ int key_limit(const DecodeParams& p, int seqlen, int t) {
-  const int n_vis = p.n_new == 0 ? 0 : (p.causal ? t + 1 : p.sq);
+// Keys of the shard visible to token t of a sequence with n_q new tokens (see the file comment), at most the capacity.
+__device__ __forceinline__ int key_limit(const DecodeParams& p, int seqlen, int n_q, int t) {
+  const int n_vis = p.n_new == 0 ? 0 : (p.causal ? t + 1 : n_q);
   const int lim = seqlen + n_vis;
   return lim < p.s_cap ? lim : p.s_cap;
+}
+
+__device__ __forceinline__ int clamp_to(int x, int lo, int hi) { return x < lo ? lo : (x > hi ? hi : x); }
+
+// Sequence b's new tokens: first packed row (x) and count (y).  Varlen offsets are clamped to [0, total_q] and counts
+// to [0, sq], so rows [x, x + y) always lie inside q, k_new / v_new and the partial buffer.
+__device__ __forceinline__ int2 q_rows(const DecodeParams& p, int b) {
+  if (p.cu_seqlens_q == nullptr) return make_int2(b * p.sq, p.sq);
+  const int lo = clamp_to(__ldg(p.cu_seqlens_q + b), 0, p.total_q);
+  const int hi = clamp_to(__ldg(p.cu_seqlens_q + b + 1), 0, p.total_q);
+  return make_int2(lo, clamp_to(hi - lo, 0, p.sq));
+}
+
+// Varlen schedule: tile slot -> (sequence b, row tile), by a prefix sum over the sequences' row-tile counts
+// ceil(n_b * G / 64), 32 sequences per step (one per lane).  Run by each warp on its own; every lane gets the same
+// answer.  False for a slot past the last real tile.
+__device__ __forceinline__ bool varlen_tile(const DecodeParams& p, int slot, int group, int& b, int& tile,
+                                            int2& rows) {
+  const int lane = threadIdx.x & 31;
+  int base = 0;  // tiles of the sequences before this step's 32
+  for (int c = 0; c < p.batch; c += 32) {
+    const int i = c + lane;
+    const int2 r = i < p.batch ? q_rows(p, i) : make_int2(0, 0);
+    const int tiles = (r.y * group + kRows - 1) / kRows;
+    int incl = tiles;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const int x = __shfl_up_sync(0xffffffffu, incl, off);
+      if (lane >= off) incl += x;
+    }
+    const int excl = base + incl - tiles;
+    const unsigned hit = __ballot_sync(0xffffffffu, slot >= excl && slot < base + incl);
+    if (hit != 0u) {
+      const int src = __ffs(hit) - 1;
+      b = c + src;
+      tile = slot - __shfl_sync(0xffffffffu, excl, src);
+      rows = make_int2(__shfl_sync(0xffffffffu, r.x, src), __shfl_sync(0xffffffffu, r.y, src));
+      return true;
+    }
+    base += __shfl_sync(0xffffffffu, incl, 31);
+  }
+  return false;
 }
 
 // TMA producer over a paged cache, run by the whole producer warp.  A 128-key tile is one page (page_size >= 128,
@@ -183,15 +231,26 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   constexpr int kSlotBytes = kTile * kD * 2;
   constexpr int kProducer = kFp8 ? 256 : 128;  // first thread of the producer warp
   const int split = blockIdx.x;
-  const int b = blockIdx.z / p.hkv, kv_head = blockIdx.z % p.hkv;
   const int group = p.hq / p.hkv;
-  const int n_rows = p.sq * group;  // packed query rows of this kv head
-  const int row0 = blockIdx.y * kRows;
+  int b, kv_head, row0;
+  int2 qr;  // the sequence's first packed query row and token count
+  if (p.cu_seqlens_q == nullptr) {
+    b = blockIdx.z / p.hkv;
+    kv_head = blockIdx.z % p.hkv;
+    row0 = blockIdx.y * kRows;
+    qr = make_int2(b * p.sq, p.sq);
+  } else {
+    int tile;
+    kv_head = blockIdx.z;
+    if (!varlen_tile(p, blockIdx.y, group, b, tile, qr)) return;  // an idle slot, in every role: nothing to write
+    row0 = tile * kRows;
+  }
+  const int n_rows = qr.y * group;  // packed query rows of this kv head
   const int rows_here = n_rows - row0 < kRows ? n_rows - row0 : kRows;
   int seqlen = p.seqlens[b];
   seqlen = seqlen < 0 ? 0 : (seqlen > p.s_cap ? p.s_cap : seqlen);
   // the last row of the tile sees the most keys (the limit never decreases with t)
-  const int kmax = key_limit(p, seqlen, (row0 + rows_here - 1) / group);
+  const int kmax = key_limit(p, seqlen, qr.y, (row0 + rows_here - 1) / group);
   const int j0 = split * p.tiles_per_split;
   int j1 = (kmax + kTile - 1) / kTile;
   if (j1 > j0 + p.tiles_per_split) j1 = j0 + p.tiles_per_split;
@@ -295,7 +354,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
     if (r < rows_here) {
       const int pr = row0 + r;
       const int t = pr / group, head = kv_head * group + pr % group;
-      val = *reinterpret_cast<const uint4*>(q + (static_cast<long long>(b) * p.sq + t) * p.q_row_stride +
+      val = *reinterpret_cast<const uint4*>(q + static_cast<long long>(qr.x + t) * p.q_row_stride +
                                             head * p.q_head_stride + 8 * c);
     }
     *reinterpret_cast<uint4*>(smem_q + (c >> 3) * kQHalfBytes + r * 128 + (((c & 7) ^ (r & 7)) << 4)) = val;
@@ -307,7 +366,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int r = r_base + 8 * h;
-    lim[h] = r < rows_here ? key_limit(p, seqlen, (row0 + r) / group) : 0;
+    lim[h] = r < rows_here ? key_limit(p, seqlen, qr.y, (row0 + r) / group) : 0;
   }
   float o[kD / 2];
 #pragma unroll
@@ -425,8 +484,13 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   }
 
   // ------------------------------------------------------------------ epilogue: O / l -> partial out, lse
-  const long long n_out = static_cast<long long>(p.batch) * p.sq * p.hq;  // rows of out
+  const long long n_out = static_cast<long long>(p.total_q) * p.hq;  // rows of out
   float* part = p.part + split * p.part_stride;
+  // lse of (head, t) at lse_row + head * lse_stride + t: (b, head, t) uniform, (head, cu[b] + t) varlen
+  const bool varlen = p.cu_seqlens_q != nullptr;
+  float* lse_row =
+      part + n_out * kD + (varlen ? static_cast<long long>(qr.x) : static_cast<long long>(b) * p.hq * p.sq);
+  const int lse_stride = varlen ? p.total_q : p.sq;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     float lt = l[h];
@@ -438,14 +502,14 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
     const int t = pr / group, head = kv_head * group + pr % group;
     float inv = lt > 0.f ? 1.0f / lt : 0.f;
     if constexpr (kFp8) inv *= p.v_descale[b * p.hkv + kv_head];
-    float* out_row = part + ((static_cast<long long>(b) * p.sq + t) * p.hq + head) * kD;
+    float* out_row = part + (static_cast<long long>(qr.x + t) * p.hq + head) * kD;
 #pragma unroll
     for (int j = 0; j < kD / 8; ++j)
       *reinterpret_cast<float2*>(out_row + 8 * j + quad_col) =
           make_float2(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
     if ((lane & 3) == 0) {
       const float lse = lt > 0.f ? (m2[h] + __log2f(lt)) * 0.6931471805599453f : -CUDART_INF_F;
-      part[n_out * kD + (static_cast<long long>(b) * p.hq + head) * p.sq + t] = lse;
+      lse_row[static_cast<long long>(head) * lse_stride + t] = lse;
     }
   }
 }
@@ -461,6 +525,13 @@ __device__ __forceinline__ long long append_row(const DecodeParams& p, int b, in
   return static_cast<long long>(page) * p.page_size + row % p.page_size;
 }
 
+// Packed row of new key t of sequence b (in k_new / v_new), or -1 past the sequence's count (varlen: one block per
+// (b, t < max_seqlen_q), and those past n_b exit).
+__device__ __forceinline__ long long new_row(const DecodeParams& p, int b, int t) {
+  const int2 r = q_rows(p, b);
+  return t < r.y ? r.x + t : -1;
+}
+
 // One block per (b, t) row of the new keys, blockIdx.y selects K or V.  16-byte chunks; rows past the capacity
 // are dropped, and so are rows whose page id lies outside the pool.
 __global__ void decode_append_kernel(uint8_t* k_cache, uint8_t* v_cache, long long row_stride_bytes,
@@ -468,10 +539,12 @@ __global__ void decode_append_kernel(uint8_t* k_cache, uint8_t* v_cache, long lo
                                      const DecodeParams p, int row_bytes) {
   const int sq = p.sq, hkv = p.hkv;
   const int b = blockIdx.x / sq, t = blockIdx.x % sq;
+  const long long in_row = new_row(p, b, t);
+  if (in_row < 0) return;
   const long long cache_row = append_row(p, b, t);
   if (cache_row < 0) return;
   uint8_t* dst = (blockIdx.y == 0 ? k_cache : v_cache) + cache_row * row_stride_bytes;
-  const uint8_t* src = (blockIdx.y == 0 ? k_new : v_new) + static_cast<long long>(blockIdx.x) * hkv * row_bytes;
+  const uint8_t* src = (blockIdx.y == 0 ? k_new : v_new) + in_row * hkv * row_bytes;
   const int chunks = row_bytes / 16;
   for (int idx = threadIdx.x; idx < hkv * chunks; idx += blockDim.x) {
     const int head = idx / chunks, c = idx % chunks;
@@ -488,10 +561,12 @@ __global__ void decode_append_e4m3_kernel(uint8_t* k_cache, uint8_t* v_cache, lo
                                           const DecodeParams p, int head_dim) {
   const int sq = p.sq, hkv = p.hkv;
   const int b = blockIdx.x / sq, t = blockIdx.x % sq;
+  const long long in_row = new_row(p, b, t);
+  if (in_row < 0) return;
   const long long cache_row = append_row(p, b, t);
   if (cache_row < 0) return;
   uint8_t* dst = (blockIdx.y == 0 ? k_cache : v_cache) + cache_row * row_stride;
-  const T* src = (blockIdx.y == 0 ? k_new : v_new) + static_cast<long long>(blockIdx.x) * hkv * head_dim;
+  const T* src = (blockIdx.y == 0 ? k_new : v_new) + in_row * hkv * head_dim;
   const float* descale = (blockIdx.y == 0 ? p.k_descale : p.v_descale) + b * hkv;
   const int chunks = head_dim / 8;
   for (int idx = threadIdx.x; idx < hkv * chunks; idx += blockDim.x) {
@@ -595,7 +670,13 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
                                                                 static_cast<const __half*>(v_new), p, head_dim);
   }
   const int row_tiles = (p.sq * (p.hq / p.hkv) + dec::kRows - 1) / dec::kRows;
-  const dim3 grid(n_splits, row_tiles, p.batch * p.hkv);
+  dim3 grid(n_splits, row_tiles, p.batch * p.hkv);
+  if (p.cu_seqlens_q != nullptr) {  // varlen: tile slots x kv heads, mapped to (sequence, row tile) on the device
+    const long long slots = decode_tile_slots(p);
+    if (slots > 65535) return "varlen decode: more than 65535 row tiles (total_q * Hq / Hkv too large)";
+    if (slots == 0) return nullptr;  // no query rows
+    grid = dim3(n_splits, static_cast<unsigned>(slots), p.hkv);
+  }
   cudaError_t err = cudaSuccess;
   auto launch = [&](auto kern, int smem, int threads) {
     err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -618,6 +699,13 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
   if (err != cudaSuccess) return cudaGetErrorString(err);
   err = cudaGetLastError();
   return err == cudaSuccess ? nullptr : cudaGetErrorString(err);
+}
+
+long long decode_tile_slots(const DecodeParams& p) {
+  const long long group = p.hq / p.hkv;
+  const long long per_seq = (p.sq * group + dec::kRows - 1) / dec::kRows;
+  const long long bound = (p.total_q * group + (dec::kRows - 1) * static_cast<long long>(p.batch)) / dec::kRows;
+  return p.batch * per_seq < bound ? p.batch * per_seq : bound;
 }
 
 const char* decode_combine_launch(const float* parts, long long part_stride, int n_parts, int batch, int sq, int hq,

@@ -51,6 +51,25 @@ def num_splits(batch: int, sq: int, hq: int, hkv: int, s_cap: int, sm_count: int
     return max(1, min(tiles, sm_count // (batch * hkv * row_tiles)))
 
 
+def tile_slots(batch: int, total_q: int, max_seqlen_q: int, hq: int, hkv: int) -> int:
+    """Row-tile slots of a varlen call's grid (per split and kv head): ``min(B * ceil(max_seqlen_q * G / 64),
+    (total_q * G + 63 * B) // 64)``, an upper bound from shapes on ``sum_b ceil(n_b * G / 64)`` for any counts
+    ``n_b <= max_seqlen_q`` summing to ``total_q``.  Each CTA maps its slot to a (sequence, row tile) on the device;
+    slots past the last real tile exit at once."""
+    g = hq // hkv
+    per_seq = -(-max_seqlen_q * g // ROWS_PER_CTA)
+    return min(batch * per_seq, (total_q * g + (ROWS_PER_CTA - 1) * batch) // ROWS_PER_CTA)
+
+
+def num_splits_varlen(batch: int, total_q: int, max_seqlen_q: int, hq: int, hkv: int, s_cap: int,
+                      sm_count: int) -> int:
+    """:func:`num_splits` for a varlen call: :func:`tile_slots` takes the place of ``B * row_tiles``.  With equal
+    counts (``total_q = B * max_seqlen_q``) it is exactly :func:`num_splits` of the uniform call."""
+    tiles = max(1, -(-s_cap // KEY_TILE))
+    slots = max(1, tile_slots(batch, total_q, max_seqlen_q, hq, hkv))
+    return max(1, min(tiles, sm_count // (slots * hkv)))
+
+
 _warned = set()
 
 
@@ -87,35 +106,48 @@ def _capacity(k_cache: Tensor, block_table: Optional[Tensor]) -> int:
 def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor, k: Optional[Tensor],
                   v: Optional[Tensor], causal: bool, softmax_scale: float, pg=None, world: int = 1,
                   splits: Optional[int] = None, block_table: Optional[Tensor] = None,
-                  k_descale: Optional[Tensor] = None, v_descale: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+                  k_descale: Optional[Tensor] = None, v_descale: Optional[Tensor] = None,
+                  cu_seqlens_q: Optional[Tensor] = None, max_seqlen_q: Optional[int] = None) -> Tuple[Tensor, Tensor]:
     """Local split-KV kernel (appending ``k`` / ``v`` first when given), then the combine over the splits and, for
     ``world > 1``, over the gathered per-rank partials.  ``splits`` overrides :func:`num_splits`.  With
     ``block_table`` the caches are page pools (see :func:`cp_flash_attn_with_kvcache`).  e4m3 caches take contiguous
-    fp32 ``(B, Hkv)`` ``k_descale`` / ``v_descale``."""
+    fp32 ``(B, Hkv)`` ``k_descale`` / ``v_descale``.  With ``cu_seqlens_q`` (and ``max_seqlen_q``) ``q`` / ``k`` /
+    ``v`` are varlen ``(total_q, H, D)`` and the result is ``out (total_q, Hq, D)``, ``lse (Hq, total_q)``."""
     C = cuda_ext.load()
-    b, sq, hq, d = q.shape
+    varlen = cu_seqlens_q is not None
+    if varlen:  # the partials are the uniform layout at batch 1, Sq = total_q
+        b = cache_seqlens.shape[0]
+        total_q, hq, d = q.shape
+        rows_b, rows_sq = 1, total_q
+    else:
+        b, sq, hq, d = q.shape
+        rows_b, rows_sq = b, sq
     q = q.contiguous()
     if k is not None:
         k, v = k.contiguous(), v.contiguous()
     if splits is None:
         dev = q.device.index if q.device.index is not None else torch.cuda.current_device()
-        splits = num_splits(b, sq, hq, k_cache.shape[2], _capacity(k_cache, block_table), _sm_count(dev))
-    n_out = b * sq * hq * d
-    size = n_out + b * hq * sq
+        s_cap, hkv = _capacity(k_cache, block_table), k_cache.shape[2]
+        if varlen:
+            splits = num_splits_varlen(b, total_q, max_seqlen_q, hq, hkv, s_cap, _sm_count(dev))
+        else:
+            splits = num_splits(b, sq, hq, hkv, s_cap, _sm_count(dev))
+    n_out = rows_b * rows_sq * hq * d
+    size = n_out + rows_b * hq * rows_sq
     parts = torch.empty((splits, size), dtype=torch.float32, device=q.device)
     C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts, block_table, k_descale,
-                 v_descale)
+                 v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0)
     cuda_ext.note_launch(2 if k is not None else 1)
     if world > 1:
         mine = torch.empty(size, dtype=torch.float32, device=q.device)
-        C.decode_combine(parts, mine[:n_out].view(b, sq, hq, d), mine[n_out:].view(b, hq, sq))
+        C.decode_combine(parts, mine[:n_out].view(rows_b, rows_sq, hq, d), mine[n_out:].view(rows_b, hq, rows_sq))
         cuda_ext.note_launch()
         parts = _gather(mine, pg, world)
     out = torch.empty(q.shape, dtype=q.dtype, device=q.device)
-    lse = torch.empty((b, hq, sq), dtype=torch.float32, device=q.device)
-    C.decode_combine(parts, out, lse)
+    lse = torch.empty((rows_b, hq, rows_sq), dtype=torch.float32, device=q.device)
+    C.decode_combine(parts, out.view(rows_b, rows_sq, hq, d), lse)
     cuda_ext.note_launch()
-    return out, lse
+    return out, (lse.view(hq, rows_sq) if varlen else lse)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -128,35 +160,61 @@ def quantize_e4m3(x: Tensor, descale: Tensor) -> Tensor:
     return (x.float() / descale[:, None]).clamp(-448, 448).to(torch.float8_e4m3fn)
 
 
+def _varlen_spans(cu_seqlens_q: Tensor, total_q: int, max_seqlen_q: int):
+    """(first row, count) of every sequence of a varlen call; ``ValueError`` for a malformed ``cu_seqlens_q``."""
+    cu = cu_seqlens_q.tolist()
+    if cu[0] != 0 or cu[-1] != total_q:
+        raise ValueError(f"cu_seqlens_q must start at 0 and end at total_q = {total_q}, not {cu[0]} ... {cu[-1]}")
+    spans = [(lo, hi - lo) for lo, hi in zip(cu[:-1], cu[1:])]
+    if any(n < 0 for _, n in spans):
+        raise ValueError("cu_seqlens_q must not decrease")
+    if any(n > max_seqlen_q for _, n in spans):
+        raise ValueError(f"cu_seqlens_q has a count above max_seqlen_q = {max_seqlen_q}")
+    return spans
+
+
 def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table=None,
-                  k_descale=None, v_descale=None):
-    b, sq, hq, d = q.shape
+                  k_descale=None, v_descale=None, cu_seqlens_q=None, max_seqlen_q=0):
+    # every sequence is a (first row, count) span of the packed rows: (b * Sq, Sq) for a uniform q
+    b = cache_seqlens.shape[0]
+    hq, d = q.shape[-2:]
+    if cu_seqlens_q is not None:
+        spans = _varlen_spans(cu_seqlens_q, q.shape[0], max_seqlen_q)
+    else:
+        sq = q.shape[1]
+        spans = [(i * sq, sq) for i in range(b)]
+        q = q.reshape(b * sq, hq, d)
+        if k is not None:
+            k, v = k.reshape(b * sq, *k.shape[2:]), v.reshape(b * sq, *v.shape[2:])
+    rows = q.shape[0]
     s_cap = _capacity(k_cache, block_table)
     lens = [max(0, min(int(x), s_cap)) for x in cache_seqlens.tolist()]
-    n_new = sq if k is not None else 0
     ps, n_pages = k_cache.shape[1], k_cache.shape[0]
     table = block_table.tolist() if block_table is not None else None
     fp8 = k_descale is not None
     if k is not None:  # rows past the capacity (or whose page is outside the pool) are dropped, as in the kernel path
         if fp8:
-            k = torch.stack([quantize_e4m3(k[i], k_descale[i]) for i in range(b)])
-            v = torch.stack([quantize_e4m3(v[i], v_descale[i]) for i in range(b)])
+            k = torch.cat([quantize_e4m3(k[lo:lo + n], k_descale[i]) for i, (lo, n) in enumerate(spans)])
+            v = torch.cat([quantize_e4m3(v[lo:lo + n], v_descale[i]) for i, (lo, n) in enumerate(spans)])
         for i, n in enumerate(lens):
-            m = min(sq, s_cap - n)
+            lo, cnt = spans[i]
+            m = min(cnt, s_cap - n)
             if table is None:
-                k_cache[i, n:n + m] = k[i, :m]
-                v_cache[i, n:n + m] = v[i, :m]
+                k_cache[i, n:n + m] = k[lo:lo + m]
+                v_cache[i, n:n + m] = v[lo:lo + m]
                 continue
             for t in range(m):
                 page = table[i][(n + t) // ps]
                 if 0 <= page < n_pages:
-                    k_cache[page, (n + t) % ps] = k[i, t]
-                    v_cache[page, (n + t) % ps] = v[i, t]
-    out = torch.zeros((b, sq, hq, d), dtype=torch.float32, device=q.device)
-    lse = torch.full((b, hq, sq), float("-inf"), dtype=torch.float32, device=q.device)
+                    k_cache[page, (n + t) % ps] = k[lo + t]
+                    v_cache[page, (n + t) % ps] = v[lo + t]
+    out = torch.zeros((rows, hq, d), dtype=torch.float32, device=q.device)
+    lse = torch.full((hq, rows), float("-inf"), dtype=torch.float32, device=q.device)
     for i, n in enumerate(lens):
+        lo, cnt = spans[i]
+        n_new = cnt if k is not None else 0
         n_keys = min(n + n_new, s_cap)
-        if n_keys == 0:
+        if n_keys == 0 or cnt == 0:
             continue
         if table is None:
             kk, vv = k_cache[i, :n_keys], v_cache[i, :n_keys]
@@ -169,17 +227,18 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
             kk, vv = kk.float() * k_descale[i][:, None], vv.float() * v_descale[i][:, None]
         # appended key u (row n + u) is visible to token t iff u <= t, i.e. row j <= t + n
         diag = n if (n_new and causal) else None
-        out[i], lse[i] = block_fwd(q[i], kk, vv, softmax_scale, diag)
+        out[lo:lo + cnt], lse[:, lo:lo + cnt] = block_fwd(q[lo:lo + cnt], kk, vv, softmax_scale, diag)
     if world > 1:
         parts = _gather(torch.cat([out.reshape(-1), lse.reshape(-1)]), pg, world)
         n_out = out.numel()
         acc_o = acc_l = None
         for r in range(world):  # rank order: the same on every rank
-            o = parts[r, :n_out].view(b * sq, hq, d)
-            l = parts[r, n_out:].view(b, hq, sq).permute(1, 0, 2).reshape(hq, b * sq)
-            acc_o, acc_l = merge_partial(acc_o, acc_l, o, l)
-        out = acc_o.view(b, sq, hq, d)
-        lse = acc_l.view(hq, b, sq).permute(1, 0, 2).contiguous()
+            acc_o, acc_l = merge_partial(acc_o, acc_l, parts[r, :n_out].view(rows, hq, d),
+                                         parts[r, n_out:].view(hq, rows))
+        out, lse = acc_o, acc_l
+    if cu_seqlens_q is None:  # back to (B, Sq, Hq, D) and (B, Hq, Sq)
+        out = out.reshape(b, sq, hq, d)
+        lse = lse.reshape(hq, b, sq).permute(1, 0, 2).contiguous()
     return out.to(q.dtype), lse
 
 
@@ -190,12 +249,13 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
 @torch.library.custom_op("rfa_b200::cp_decode", mutates_args=("k_cache", "v_cache"))
 def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor, k: Optional[Tensor],
               v: Optional[Tensor], append_rank: int, softmax_scale: float, causal: bool, group: str,
-              block_table: Optional[Tensor], k_descale: Optional[Tensor],
-              v_descale: Optional[Tensor]) -> Tuple[Tensor, Tensor]:
+              block_table: Optional[Tensor], k_descale: Optional[Tensor], v_descale: Optional[Tensor],
+              cu_seqlens_q: Optional[Tensor], max_seqlen_q: int) -> Tuple[Tensor, Tensor]:
     """q (B, Sq, Hq, D) -> (out (B, Sq, Hq, D) in q.dtype, lse (B, Hq, Sq) fp32).  ``k`` / ``v`` are appended to
     the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's name ("" = world);
     with ``block_table`` the caches are this rank's page pools; e4m3 caches come with contiguous fp32 (B, Hkv)
-    ``k_descale`` / ``v_descale``."""
+    ``k_descale`` / ``v_descale``.  With ``cu_seqlens_q`` q / k / v are varlen (total_q, H, D), out is
+    (total_q, Hq, D) and lse (Hq, total_q); ``max_seqlen_q`` bounds the counts (0 when uniform)."""
     pg = resolve_group(group)
     rank, world = group_info(pg)
     if k is not None and not 0 <= append_rank < world:
@@ -204,14 +264,18 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
         k = v = None
     if _kernel_takes(q):
         return kernel_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world,
-                             block_table=block_table, k_descale=k_descale, v_descale=v_descale)
+                             block_table=block_table, k_descale=k_descale, v_descale=v_descale,
+                             cu_seqlens_q=cu_seqlens_q, max_seqlen_q=max_seqlen_q)
     return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table,
-                         k_descale, v_descale)
+                         k_descale, v_descale, cu_seqlens_q, max_seqlen_q)
 
 
 @cp_decode.register_fake
 def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group, block_table, k_descale,
-      v_descale):
+      v_descale, cu_seqlens_q, max_seqlen_q):
+    if cu_seqlens_q is not None:
+        total_q, hq, _ = q.shape
+        return q.new_empty(q.shape), q.new_empty((hq, total_q), dtype=torch.float32)
     b, sq, hq, _ = q.shape
     return q.new_empty(q.shape), q.new_empty((b, hq, sq), dtype=torch.float32)
 
@@ -220,8 +284,7 @@ def _valid_page_size(ps: int) -> bool:
     return ps in (16, 32, 64) or (ps > 0 and ps % KEY_TILE == 0)
 
 
-def _check_block_table(q, k_cache, v_cache, block_table):
-    b = q.shape[0]
+def _check_block_table(q, k_cache, v_cache, block_table, b):
     if (block_table.dtype != torch.int32 or block_table.dim() != 2 or block_table.shape[0] != b
             or block_table.shape[1] < 1 or block_table.stride(1) != 1):
         raise ValueError("block_table must be a (B, max_blocks) int32 tensor with stride(1) == 1")
@@ -252,8 +315,8 @@ def _check_descale(name, x, q, b, hkv):
 
 def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=None, append_rank=None,
                                softmax_scale=None, causal=True, return_softmax_lse=False, group=None, *,
-                               block_table=None, k_descale=None, v_descale=None, window_size=(-1, -1),
-                               alibi_slopes=None):
+                               block_table=None, k_descale=None, v_descale=None, cu_seqlens_q=None,
+                               max_seqlen_q=None, window_size=(-1, -1), alibi_slopes=None):
     """Decode attention of new query tokens against a KV cache sharded over ``group`` (modelled on flash-attn's
     ``flash_attn_with_kvcache``).  Inference only: no gradient.
 
@@ -286,6 +349,20 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
       and must be ``None`` without them; it must be the same int on every rank (e.g. ``step % world``).
     * Query token ``t`` sees every valid cached key of every rank and, with ``causal=True``, the appended keys
       ``0..t`` of its own call (flash-attn's bottom-right alignment); with ``causal=False`` all ``Sq`` of them.
+    * Varlen queries (flash-attn's ``cu_seqlens_q`` / ``max_seqlen_q``): every sequence may bring a different
+      number of new tokens.  ``q`` is then ``(total_q, Hq, D)``, and sequence ``b`` owns rows
+      ``cu_seqlens_q[b]:cu_seqlens_q[b + 1]`` (0 rows is allowed); ``B`` is ``cache_seqlens.shape[0]`` and
+      ``cu_seqlens_q`` a contiguous ``(B + 1,)`` int32 tensor on q's device, the same on every rank.  ``max_seqlen_q``
+      (a host int >= 1, required with ``cu_seqlens_q`` and rejected without it) bounds every count.  ``k`` / ``v``
+      are ``(total_q, Hkv, D)`` with the same row ranges; sequence ``b``'s ``n_b`` rows go to cache rows
+      ``[cache_seqlens[b], cache_seqlens[b] + n_b)``.  ``out`` is ``(total_q, Hq, D)`` and ``softmax_lse``
+      ``(Hq, total_q)`` (flash-attn's varlen layout).  Masking is per sequence, as above, with ``n_b`` for ``Sq``.
+      Composes with ``block_table`` and e4m3 caches.  The kernel path reads ``cu_seqlens_q`` on the device only (a
+      step with fixed ``total_q`` / ``max_seqlen_q`` can be captured in a CUDA graph, and a replay uses the current
+      contents) and does not validate it: malformed values give an undefined result for the affected rows, but no
+      access outside ``q``, ``k``, ``v`` or the caches.  The dense path raises ``ValueError`` for them
+      (``cu_seqlens_q[0] != 0``, a decreasing entry, ``cu_seqlens_q[B] != total_q``, a count above
+      ``max_seqlen_q``).  Long chunks are correct but not efficient: every 64-row tile reads the whole shard.
     * Returns ``out`` ``(B, Sq, Hq, D)`` in q.dtype, and ``softmax_lse`` ``(B, Hq, Sq)`` fp32 when
       ``return_softmax_lse``.  Both are bitwise identical on every rank.
     * ``window_size``, ``alibi_slopes``, ``D > 128`` and ``Hq % Hkv != 0`` raise ``ValueError``.  The sm_90a kernel
@@ -298,12 +375,36 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
         raise ValueError("cp_flash_attn_with_kvcache: sliding windows are not supported in decode")
     if alibi_slopes is not None:
         raise ValueError("cp_flash_attn_with_kvcache: alibi_slopes are not supported in decode")
-    if q.dim() != 4 or k_cache.dim() != 4 or tuple(k_cache.shape) != tuple(v_cache.shape):
+    varlen = cu_seqlens_q is not None
+    if varlen:
+        if q.dim() != 3:
+            raise ValueError(f"with cu_seqlens_q, q must be (total_q, Hq, D), not {tuple(q.shape)}")
+        if max_seqlen_q is None:
+            raise ValueError("max_seqlen_q is required with cu_seqlens_q")
+        if isinstance(max_seqlen_q, bool) or not isinstance(max_seqlen_q, int) or max_seqlen_q < 1:
+            raise ValueError(f"max_seqlen_q must be a host int >= 1, not {max_seqlen_q!r}")
+        if not isinstance(cache_seqlens, Tensor) or cache_seqlens.dim() != 1:
+            raise ValueError("cache_seqlens must be a (B,) int32 tensor on q's device")
+    else:
+        if max_seqlen_q is not None:
+            raise ValueError("max_seqlen_q is only taken with cu_seqlens_q")
+        if q.dim() == 3:
+            raise ValueError("a 3-D (total_q, Hq, D) q needs cu_seqlens_q")
+    if q.dim() != (3 if varlen else 4) or k_cache.dim() != 4 or tuple(k_cache.shape) != tuple(v_cache.shape):
         raise ValueError("q must be (B, Sq, Hq, D) and k_cache / v_cache the same (B, S_cap, Hkv, D) shape")
-    b, sq, hq, d = q.shape
+    if varlen:
+        b, sq = cache_seqlens.shape[0], max_seqlen_q
+        total_q, hq, d = q.shape
+    else:
+        b, sq, hq, d = q.shape
     hkv = k_cache.shape[2]
     if (block_table is None and k_cache.shape[0] != b) or k_cache.shape[3] != d or sq < 1:
         raise ValueError(f"q {tuple(q.shape)} does not match the cache {tuple(k_cache.shape)}")
+    if varlen and (not isinstance(cu_seqlens_q, Tensor) or cu_seqlens_q.dtype != torch.int32
+                   or tuple(cu_seqlens_q.shape) != (b + 1,) or not cu_seqlens_q.is_contiguous()):
+        raise ValueError(f"cu_seqlens_q must be a contiguous (B + 1,) = ({b + 1},) int32 tensor")
+    if varlen and cu_seqlens_q.device != q.device:
+        raise ValueError("cu_seqlens_q must be on q's device")
     if q.element_size() == 1:
         raise ValueError("cp_flash_attn_with_kvcache: fp8 queries are not supported")
     if k_cache.element_size() == 1 or v_cache.element_size() == 1:
@@ -329,18 +430,22 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
             or cache_seqlens.device != q.device):
         raise ValueError("cache_seqlens must be a (B,) int32 tensor on q's device")
     if block_table is not None:
-        _check_block_table(q, k_cache, v_cache, block_table)
+        _check_block_table(q, k_cache, v_cache, block_table, b)
     if (k is None) != (v is None):
         raise ValueError("pass both k and v, or neither")
     if k is not None:
         if append_rank is None:
             raise ValueError("append_rank is required when k / v are given")
         for t in (k, v):
-            if tuple(t.shape) != (b, sq, hkv, d) or t.dtype != q.dtype:
+            if varlen and (tuple(t.shape) != (total_q, hkv, d) or t.dtype != q.dtype):
+                raise ValueError(f"with cu_seqlens_q, k / v must be (total_q, Hkv, D) = {(total_q, hkv, d)} in "
+                                 "q's dtype")
+            if not varlen and (tuple(t.shape) != (b, sq, hkv, d) or t.dtype != q.dtype):
                 raise ValueError(f"k / v must be (B, Sq, Hkv, D) = {(b, sq, hkv, d)} in q's dtype")
     elif append_rank is not None:
         raise ValueError("append_rank must be None when no k / v are given")
     scale = float(softmax_scale) if softmax_scale is not None else d ** -0.5
     out, lse = cp_decode(q, k_cache, v_cache, cache_seqlens, k, v, -1 if append_rank is None else int(append_rank),
-                         scale, bool(causal), group_name(group), block_table, k_descale, v_descale)
+                         scale, bool(causal), group_name(group), block_table, k_descale, v_descale, cu_seqlens_q,
+                         max_seqlen_q if varlen else 0)
     return (out, lse) if return_softmax_lse else out
