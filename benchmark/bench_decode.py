@@ -15,11 +15,16 @@ With ``--mixed-chunk C`` every configuration also times, in the same loop, a var
 sequence 0 brings C new tokens and the others 1, the uniform call padded to Sq = C (what a caller without varlen
 must do) and the uniform Sq = 1 call (the pure-decode floor), with the K + V bytes the varlen and padded calls stream
 (every 64-row tile streams its sequence's shard).
+With ``--rotary`` every configuration also times, in the same loop, a RoPE decode step that appends the new k / v
+(the shard then holds the cache length): the fused call (``rotary_cos`` / ``rotary_sin``, non-interleaved, rotary_dim
+= head_dim), the same step done without it (``apply_rotary`` on q and k with torch ops, then a plain call), and the
+plain call alone; and reports whether the fused and unfused outputs are bitwise equal.
 
     python benchmark/bench_decode.py                      # B in {1, 8}, caches of 32K..512K tokens per rank
     python benchmark/bench_decode.py --page-size 16       # also the paged kernel, pages of 16 rows
     python benchmark/bench_decode.py --kv-dtype e4m3      # also the fp8-cache kernel
     python benchmark/bench_decode.py --mixed-chunk 64     # also a ragged batch: one 64-token chunk + decodes
+    python benchmark/bench_decode.py --rotary             # also the fused RoPE step against the unfused one
     torchrun --nproc-per-node 2 benchmark/bench_decode.py
     python benchmark/bench_decode.py --dry-run            # shapes and byte counts only (no GPU)
 """
@@ -55,6 +60,8 @@ def parse_args(argv=None):
     ap.add_argument("--mixed-chunk", type=int, default=None, metavar="C",
                     help="also time a varlen batch (sequence 0 brings C tokens, the others 1) against the uniform "
                          "call padded to Sq = C and the uniform Sq = 1 call")
+    ap.add_argument("--rotary", action="store_true",
+                    help="also time a RoPE step: the fused call, the torch rotation + a plain call, the plain call")
     ap.add_argument("--dry-run", action="store_true")
     return ap.parse_args(argv)
 
@@ -81,6 +88,8 @@ def shapes(args, sm_count):
                            varlen_splits=dec.num_splits_varlen(b, total_q, c, args.hq, args.hkv, s, sm_count),
                            padded_splits=dec.num_splits(b, c, args.hq, args.hkv, s, sm_count),
                            varlen_kv_bytes=(chunk_tiles + b - 1) * shard, padded_kv_bytes=b * chunk_tiles * shard)
+            if args.rotary:  # positions cache_tokens - Sq + t of a table with one row per cached token
+                cfg.update(rotary_dim=args.head_dim, rotary_interleaved=False, seqlen_ro=s)
             yield cfg
 
 
@@ -199,6 +208,28 @@ def main():
             def decode_only():
                 return dec.kernel_decode(q_one, kc, vc, sl, None, None, True, scale)
 
+        if args.rotary:  # append Sq new tokens at rows [s - Sq, s), rotated at those positions
+            k_new = torch.randn(b, args.sq, args.hkv, d, device=dev, dtype=torch.bfloat16)
+            v_new = torch.randn_like(k_new)
+            sl_app = torch.full((b,), s - args.sq, dtype=torch.int32, device=dev)
+            inv = 10000.0 ** (-torch.arange(0, d, 2, dtype=torch.float64, device=dev) / d)
+            ang = torch.arange(s, dtype=torch.float64, device=dev)[:, None] * inv[None]
+            cos, sin = ang.cos().to(torch.bfloat16), ang.sin().to(torch.bfloat16)
+            del ang
+            pos = sl_app.long()[:, None] + torch.arange(args.sq, device=dev)[None]  # (B, Sq)
+
+            def rot_fused():
+                return dec.kernel_decode(q, kc, vc, sl_app, k_new, v_new, True, scale, rotary_cos=cos,
+                                         rotary_sin=sin, rotary_seqlens=sl_app, rotary_interleaved=False)
+
+            def rot_unfused():  # the step without rotary_cos: rotate q and k with torch ops, then a plain call
+                qr = dec.apply_rotary(q, cos, sin, pos, False)
+                kr = dec.apply_rotary(k_new, cos, sin, pos, False)
+                return dec.kernel_decode(qr, kc, vc, sl_app, kr, v_new, True, scale)
+
+            def rot_plain():
+                return dec.kernel_decode(q, kc, vc, sl_app, k_new, v_new, True, scale)
+
         # SDPA reads the same shard through (B, H, S, D) views
         qt, kt, vt = q.transpose(1, 2), kc.transpose(1, 2), vc.transpose(1, 2)
 
@@ -213,6 +244,7 @@ def main():
             if args.page_size:
                 rows["paged_fp8"] = []
         mixed_rows = {"mixed_varlen": [], "mixed_padded": [], "mixed_decode_only": []}
+        rot_rows = {"rotary_fused": [], "rotary_unfused": [], "rotary_plain": []}
         sdpa_err = None
         for _ in range(3):  # alternate them in one run
             rows["ours"].append(time_us(ours, args.iters, args.warmup))
@@ -220,6 +252,10 @@ def main():
                 mixed_rows["mixed_varlen"].append(time_us(mixed, args.iters, args.warmup))
                 mixed_rows["mixed_padded"].append(time_us(padded, args.iters, args.warmup))
                 mixed_rows["mixed_decode_only"].append(time_us(decode_only, args.iters, args.warmup))
+            if args.rotary:
+                rot_rows["rotary_fused"].append(time_us(rot_fused, args.iters, args.warmup))
+                rot_rows["rotary_unfused"].append(time_us(rot_unfused, args.iters, args.warmup))
+                rot_rows["rotary_plain"].append(time_us(rot_plain, args.iters, args.warmup))
             if args.page_size:
                 rows["paged"].append(time_us(paged, args.iters, args.warmup))
             if fp8:
@@ -252,6 +288,13 @@ def main():
             v_out, p_out = mixed()[0], padded()[0]
             res["mixed_chunk_rows_equal_padded"] = torch.equal(v_out[:c], p_out[0]) if \
                 cfg["varlen_splits"] == cfg["padded_splits"] else None
+        if args.rotary:
+            for k, ts in rot_rows.items():
+                res[f"{k}_us"] = round(min(ts), 2)
+                res[f"{k}_us_all"] = [round(t, 2) for t in ts]
+            res["rotary_fused_over_plain"] = round(res["rotary_fused_us"] / res["rotary_plain_us"], 3)
+            res["rotary_speedup_vs_unfused"] = round(res["rotary_unfused_us"] / res["rotary_fused_us"], 3)
+            res["rotary_fused_equal_unfused"] = all(torch.equal(x, y) for x, y in zip(rot_fused(), rot_unfused()))
         if args.page_size:
             res["paged_equal_contiguous"] = all(torch.equal(x, y) for x, y in zip(paged(), ours()))
         if fp8:
@@ -279,6 +322,8 @@ def main():
         del q, kc, vc
         if args.mixed_chunk:
             del q_pad, q_var, q_one
+        if args.rotary:
+            del k_new, v_new, cos, sin
         if args.page_size:
             del pk, pv
         if fp8:

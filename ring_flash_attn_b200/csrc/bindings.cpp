@@ -405,11 +405,15 @@ at::Tensor lse_unflatten(const at::Tensor& lse, const at::Tensor& cu, int64_t ma
 // v_descale fp32 (B, Hkv) contiguous on q's device: the cache then holds x / descale[b, kv head].  With cu_seqlens_q
 // (B + 1,) int32 (B = seqlens.numel()), q is varlen (total_q, Hq, D), k_new / v_new (total_q, Hkv, D), part fp32
 // (n_splits, total_q*Hq*D + Hq*total_q), and max_seqlen_q >= 1 bounds every count; cu_seqlens_q is not validated.
+// With rotary_cos / rotary_sin (seqlen_ro, rotary_dim / 2) contiguous in q's dtype and rotary_seqlens (B,) int32,
+// q and the appended k are rotated (see DecodeParams); rotary_seqlens is read on the device only.
 void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
                 const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
                 double scale, at::Tensor& part, const c10::optional<at::Tensor>& block_table,
                 const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale,
-                const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q) {
+                const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q,
+                const c10::optional<at::Tensor>& rotary_cos, const c10::optional<at::Tensor>& rotary_sin,
+                const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved) {
   const c10::cuda::CUDAGuard guard(q_in.device());
   const bool varlen = cu_seqlens_q.has_value();
   TORCH_CHECK(q_in.dim() == (varlen ? 3 : 4), "decode_fwd: q must be (B, Sq, Hq, D), or (total_q, Hq, D) with "
@@ -511,6 +515,30 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
                   "decode_fwd: fp8 descales must be contiguous fp32 (B, Hkv) on q's device");
     p.k_descale = k_descale->data_ptr<float>();
     p.v_descale = v_descale->data_ptr<float>();
+  }
+  TORCH_CHECK(rotary_cos.has_value() == rotary_sin.has_value() && rotary_cos.has_value() == rotary_seqlens.has_value(),
+              "decode_fwd: rotary needs rotary_cos, rotary_sin and rotary_seqlens together");
+  if (rotary_cos.has_value()) {
+    const at::Tensor& rc = *rotary_cos;
+    const at::Tensor& rs = *rotary_sin;
+    TORCH_CHECK(rc.dim() == 2 && rc.sizes() == rs.sizes() && rc.size(0) >= 1 && rc.is_contiguous() &&
+                    rs.is_contiguous() && rc.scalar_type() == q.scalar_type() &&
+                    rs.scalar_type() == q.scalar_type() && rc.device() == q.device() && rs.device() == q.device(),
+                "decode_fwd: rotary_cos / rotary_sin must be contiguous (seqlen_ro, rotary_dim / 2) in q's dtype on "
+                "q's device");
+    TORCH_CHECK(rc.size(1) >= 8 && rc.size(1) % 8 == 0 && 2 * rc.size(1) <= d,
+                "decode_fwd: rotary_dim must be a positive multiple of 16, at most head_dim");
+    TORCH_CHECK(rc.size(0) < (int64_t(1) << 31), "decode_fwd: seqlen_ro must be below 2^31");
+    const at::Tensor& rsl = *rotary_seqlens;
+    TORCH_CHECK(rsl.scalar_type() == at::kInt && rsl.device() == q.device() && rsl.is_contiguous() && rsl.dim() == 1 &&
+                    rsl.numel() == B,
+                "decode_fwd: rotary_seqlens must be (B,) int32 contiguous on q's device");
+    p.rotary_cos = rc.data_ptr();
+    p.rotary_sin = rs.data_ptr();
+    p.rotary_seqlens = rsl.data_ptr<int>();
+    p.rotary_half = static_cast<int>(rc.size(1));
+    p.seqlen_ro = static_cast<int>(rc.size(0));
+    p.rotary_interleaved = rotary_interleaved ? 1 : 0;
   }
   const TensorView kv{k_cache.data_ptr(), cache_rows, static_cast<int>(hkv), k_cache.stride(1), k_cache.stride(2)};
   const TensorView vv{v_cache.data_ptr(), cache_rows, static_cast<int>(hkv), v_cache.stride(1), v_cache.stride(2)};

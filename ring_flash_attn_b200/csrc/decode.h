@@ -37,6 +37,16 @@ struct DecodeParams {
   // e4m3 caches: the cache holds x / descale, per (sequence, kv head); nullptr for bf16 / fp16 caches
   const float* k_descale;  // (B, Hkv) contiguous
   const float* v_descale;
+  // Rotary embeddings of the new tokens; rotary_cos == nullptr: none.  Columns [0, 2 * rotary_half) of q and of the
+  // appended k are rotated (pairs (i, i + rotary_half), or (2i, 2i + 1) when interleaved) at position
+  // rotary_seqlens[b] + t for key t, and for query token t the same when causal, rotary_seqlens[b] otherwise.
+  // Positions are clamped to [0, seqlen_ro - 1], so a bad rotary_seqlens never reads outside the tables.
+  const void* rotary_cos;    // (seqlen_ro, rotary_half) contiguous, in q's dtype
+  const void* rotary_sin;
+  const int* rotary_seqlens;  // (B,) first new token's position; read on the device only
+  int rotary_half;            // rotary_dim / 2, a multiple of 8
+  int seqlen_ro;
+  int rotary_interleaved;
 };
 
 // Appends k_new / v_new (B, Sq, Hkv, D), contiguous, in q's dtype, at rows [seqlens[b], seqlens[b] + Sq) of the
@@ -44,7 +54,8 @@ struct DecodeParams {
 // runs the split-KV kernel.  k_new == nullptr: attention only.  cache_dtype is dtype, or kDtypeE4M3 with
 // p.k_descale / p.v_descale set: the append then stores e4m3(x / descale), saturated to +-448.  Varlen: k_new / v_new
 // are (total_q, Hkv, D) and sequence b's n_b rows go to [seqlens[b], seqlens[b] + n_b); the grid is
-// (n_splits, decode_tile_slots(p), Hkv), each slot mapped to a (sequence, row tile) on the device.
+// (n_splits, decode_tile_slots(p), Hkv), each slot mapped to a (sequence, row tile) on the device.  With
+// p.rotary_cos set, q is rotated as the kernel loads it and k_new before it is stored (see DecodeParams).
 const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_cache, const TensorView& v_cache,
                               const void* k_new, const void* v_new, const DecodeParams& p, int n_splits, int head_dim,
                               cudaStream_t stream);

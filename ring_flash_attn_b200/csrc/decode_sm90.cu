@@ -21,6 +21,10 @@
 // its (sequence, row tile) by a warp-wide prefix sum over cu, and slots past the last real tile exit at once.
 // Everything after that mapping is the uniform code with the sequence's own row base and count.
 //
+// Rotary embeddings (rotary_cos set): the compute warpgroup rotates the 16-byte chunks of each Q row below rotary_dim
+// as it loads the Q tile, before the key loop, and the append kernels rotate K before they store it.  The key loop,
+// the producer, the converter and the combine do not see it.
+//
 // Visibility: key j of the shard is visible to query token t iff j < seqlens[b] + n_vis(t), where n_vis(t) counts
 // the keys this call appended to this shard that t may see (0 on every rank but the append rank; t + 1 when causal,
 // the sequence's token count otherwise).  Cache rows at or past that limit are never read into a result: their K
@@ -86,6 +90,63 @@ __device__ __forceinline__ int2 q_rows(const DecodeParams& p, int b) {
   const int lo = clamp_to(__ldg(p.cu_seqlens_q + b), 0, p.total_q);
   const int hi = clamp_to(__ldg(p.cu_seqlens_q + b + 1), 0, p.total_q);
   return make_int2(lo, clamp_to(hi - lo, 0, p.sq));
+}
+
+// Rotary position of new token t of sequence b (t = 0 for every query token of a non-causal call), clamped to the
+// tables: a bad rotary_seqlens gives a wrong rotation, never a read outside them.
+__device__ __forceinline__ int rotary_pos(const DecodeParams& p, int b, int t) {
+  const long long x = static_cast<long long>(__ldg(p.rotary_seqlens + b)) + t;
+  return x < 0 ? 0 : (x >= p.seqlen_ro ? p.seqlen_ro - 1 : static_cast<int>(x));
+}
+
+template <typename T>
+__device__ __forceinline__ T round_to(float x) {
+  if constexpr (std::is_same_v<T, __half>) return __float2half_rn(x);
+  else return __float2bfloat16_rn(x);
+}
+
+// The rotated 16-byte chunk c (elements 8c .. 8c + 7, all below rotary_dim) of a q / k row `row` whose chunk c holds
+// `val`, at table row pos: y = x * cos -+ x_pair * sin, every operand widened to fp32, each product and the sum rounded
+// to fp32 (no FMA), the result rounded to nearest even into T.  Interleaved, the pairs (2i, 2i + 1) lie inside the
+// chunk; otherwise chunk c pairs with the chunk rotary_half / 8 away, 16-byte aligned since rotary_half % 8 == 0.
+template <typename T>
+__device__ __forceinline__ uint4 rotate_chunk(uint4 val, const T* row, int c, int pos, const DecodeParams& p) {
+  const int h = p.rotary_half;
+  const T* cos_row = static_cast<const T*>(p.rotary_cos) + static_cast<long long>(pos) * h;
+  const T* sin_row = static_cast<const T*>(p.rotary_sin) + static_cast<long long>(pos) * h;
+  const T* x = reinterpret_cast<const T*>(&val);
+  uint4 res;
+  T* y = reinterpret_cast<T*>(&res);
+  if (p.rotary_interleaved) {
+    const uint2 cr = __ldg(reinterpret_cast<const uint2*>(cos_row + 4 * c));
+    const uint2 sr = __ldg(reinterpret_cast<const uint2*>(sin_row + 4 * c));
+    const T* cv = reinterpret_cast<const T*>(&cr);
+    const T* sv = reinterpret_cast<const T*>(&sr);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float x0 = static_cast<float>(x[2 * i]), x1 = static_cast<float>(x[2 * i + 1]);
+      const float co = static_cast<float>(cv[i]), si = static_cast<float>(sv[i]);
+      y[2 * i] = round_to<T>(__fsub_rn(__fmul_rn(x0, co), __fmul_rn(x1, si)));
+      y[2 * i + 1] = round_to<T>(__fadd_rn(__fmul_rn(x1, co), __fmul_rn(x0, si)));
+    }
+  } else {
+    const int half_chunks = h / 8;
+    const bool first = c < half_chunks;  // y[i] = x[i] c - x[i + h] s, else y[i + h] = x[i + h] c + x[i] s
+    const int tc = first ? c : c - half_chunks;  // chunk of the tables
+    const uint4 pr = *reinterpret_cast<const uint4*>(row + 8 * (first ? c + half_chunks : tc));
+    const uint4 cr = __ldg(reinterpret_cast<const uint4*>(cos_row + 8 * tc));
+    const uint4 sr = __ldg(reinterpret_cast<const uint4*>(sin_row + 8 * tc));
+    const T* xp = reinterpret_cast<const T*>(&pr);
+    const T* cv = reinterpret_cast<const T*>(&cr);
+    const T* sv = reinterpret_cast<const T*>(&sr);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float a = __fmul_rn(static_cast<float>(x[i]), static_cast<float>(cv[i]));
+      const float b = __fmul_rn(static_cast<float>(xp[i]), static_cast<float>(sv[i]));
+      y[i] = round_to<T>(first ? __fsub_rn(a, b) : __fadd_rn(a, b));
+    }
+  }
+  return res;
 }
 
 // Varlen schedule: tile slot -> (sequence b, row tile), by a prefix sum over the sequences' row-tile counts
@@ -345,7 +406,8 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   const int quad_col = 2 * (lane & 3);                // its columns: 8 j + quad_col + {0, 1}
   const T* q = reinterpret_cast<const T*>(p.q);
 
-  // Q tile: packed rows in the 128-byte swizzled K-major layout TMA would write; rows past the group are zero
+  // Q tile: packed rows in the 128-byte swizzled K-major layout TMA would write; rows past the group are zero.  With
+  // rotary, chunks below rotary_dim are rotated on the way (token t's position; the first token's when not causal).
   constexpr int kChunks = kD / 8;  // 16-byte chunks per row
 #pragma unroll 4
   for (int idx = tid; idx < kRows * kChunks; idx += 128) {
@@ -354,8 +416,10 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
     if (r < rows_here) {
       const int pr = row0 + r;
       const int t = pr / group, head = kv_head * group + pr % group;
-      val = *reinterpret_cast<const uint4*>(q + static_cast<long long>(qr.x + t) * p.q_row_stride +
-                                            head * p.q_head_stride + 8 * c);
+      const T* q_row = q + static_cast<long long>(qr.x + t) * p.q_row_stride + head * p.q_head_stride;
+      val = *reinterpret_cast<const uint4*>(q_row + 8 * c);
+      if (p.rotary_cos != nullptr && c < p.rotary_half / 4)
+        val = rotate_chunk<T>(val, q_row, c, rotary_pos(p, b, p.causal ? t : 0), p);
     }
     *reinterpret_cast<uint4*>(smem_q + (c >> 3) * kQHalfBytes + r * 128 + (((c & 7) ^ (r & 7)) << 4)) = val;
   }
@@ -533,7 +597,9 @@ __device__ __forceinline__ long long new_row(const DecodeParams& p, int b, int t
 }
 
 // One block per (b, t) row of the new keys, blockIdx.y selects K or V.  16-byte chunks; rows past the capacity
-// are dropped, and so are rows whose page id lies outside the pool.
+// are dropped, and so are rows whose page id lies outside the pool.  With rotary, the K chunks below rotary_dim are
+// rotated as elements of T (at position rotary_seqlens[b] + t) before they are stored; everything else is a byte copy.
+template <typename T>
 __global__ void decode_append_kernel(uint8_t* k_cache, uint8_t* v_cache, long long row_stride_bytes,
                                      long long head_stride_bytes, const uint8_t* k_new, const uint8_t* v_new,
                                      const DecodeParams p, int row_bytes) {
@@ -545,16 +611,20 @@ __global__ void decode_append_kernel(uint8_t* k_cache, uint8_t* v_cache, long lo
   if (cache_row < 0) return;
   uint8_t* dst = (blockIdx.y == 0 ? k_cache : v_cache) + cache_row * row_stride_bytes;
   const uint8_t* src = (blockIdx.y == 0 ? k_new : v_new) + in_row * hkv * row_bytes;
+  const bool rotate = blockIdx.y == 0 && p.rotary_cos != nullptr;
+  const int pos = rotate ? rotary_pos(p, b, t) : 0;
   const int chunks = row_bytes / 16;
   for (int idx = threadIdx.x; idx < hkv * chunks; idx += blockDim.x) {
     const int head = idx / chunks, c = idx % chunks;
-    *reinterpret_cast<uint4*>(dst + head * head_stride_bytes + 16 * c) =
-        *reinterpret_cast<const uint4*>(src + static_cast<long long>(head) * row_bytes + 16 * c);
+    const uint8_t* in = src + static_cast<long long>(head) * row_bytes;
+    uint4 val = *reinterpret_cast<const uint4*>(in + 16 * c);
+    if (rotate && c < p.rotary_half / 4) val = rotate_chunk<T>(val, reinterpret_cast<const T*>(in), c, pos, p);
+    *reinterpret_cast<uint4*>(dst + head * head_stride_bytes + 16 * c) = val;
   }
 }
 
 // The same into e4m3 caches: x / descale[b, head] (IEEE division), saturated to +-448 and rounded to nearest even
-// (NaN stays NaN), 8 values per step.
+// (NaN stays NaN), 8 values per step.  With rotary, K is first rotated and rounded to T, as in decode_append_kernel.
 template <typename T>
 __global__ void decode_append_e4m3_kernel(uint8_t* k_cache, uint8_t* v_cache, long long row_stride,
                                           long long head_stride, const T* k_new, const T* v_new,
@@ -568,11 +638,15 @@ __global__ void decode_append_e4m3_kernel(uint8_t* k_cache, uint8_t* v_cache, lo
   uint8_t* dst = (blockIdx.y == 0 ? k_cache : v_cache) + cache_row * row_stride;
   const T* src = (blockIdx.y == 0 ? k_new : v_new) + in_row * hkv * head_dim;
   const float* descale = (blockIdx.y == 0 ? p.k_descale : p.v_descale) + b * hkv;
+  const bool rotate = blockIdx.y == 0 && p.rotary_cos != nullptr;
+  const int pos = rotate ? rotary_pos(p, b, t) : 0;
   const int chunks = head_dim / 8;
   for (int idx = threadIdx.x; idx < hkv * chunks; idx += blockDim.x) {
     const int head = idx / chunks, c = idx % chunks;
     const float ds = descale[head];
-    const uint4 raw = *reinterpret_cast<const uint4*>(src + static_cast<long long>(head) * head_dim + 8 * c);
+    const T* in = src + static_cast<long long>(head) * head_dim;
+    uint4 raw = *reinterpret_cast<const uint4*>(in + 8 * c);
+    if (rotate && c < p.rotary_half / 4) raw = rotate_chunk<T>(raw, in, c, pos, p);
     const T* x = reinterpret_cast<const T*>(&raw);
     float f[8];
 #pragma unroll
@@ -644,6 +718,12 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
     if (!size_ok) return "page_size must be 16, 32, 64 or a positive multiple of 128";
     if (p.block_table == nullptr) return "a paged cache needs a block table";
   }
+  if (p.rotary_cos != nullptr) {
+    if (p.rotary_sin == nullptr || p.rotary_seqlens == nullptr) return "rotary needs cos, sin and rotary_seqlens";
+    if (p.rotary_half <= 0 || p.rotary_half % 8 != 0 || 2 * p.rotary_half > head_dim)
+      return "rotary_dim must be a positive multiple of 16, at most head_dim";
+    if (p.seqlen_ro < 1) return "the rotary tables must have at least one row";
+  }
   // a paged cache's tensor maps cover the whole pool; a box is at most one page
   const int box_rows = p.page_size != 0 && p.page_size < dec::kTile ? p.page_size : dec::kTile;
   // e4m3 rows are head_dim bytes: one 128-byte swizzle span at head_dim 128, one 64-byte span at 64
@@ -656,10 +736,14 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
     const dim3 agrid(p.batch * p.sq, 2);
     uint8_t* kc = static_cast<uint8_t*>(k_cache.ptr);
     uint8_t* vc = static_cast<uint8_t*>(v_cache.ptr);
-    if (!fp8)
-      dec::decode_append_kernel<<<agrid, 128, 0, stream>>>(kc, vc, k_cache.row_stride * 2, k_cache.head_stride * 2,
-                                                           static_cast<const uint8_t*>(k_new),
-                                                           static_cast<const uint8_t*>(v_new), p, head_dim * 2);
+    const uint8_t* kn = static_cast<const uint8_t*>(k_new);
+    const uint8_t* vn = static_cast<const uint8_t*>(v_new);
+    if (!fp8 && dtype == kDtypeBF16)
+      dec::decode_append_kernel<__nv_bfloat16><<<agrid, 128, 0, stream>>>(
+          kc, vc, k_cache.row_stride * 2, k_cache.head_stride * 2, kn, vn, p, head_dim * 2);
+    else if (!fp8)
+      dec::decode_append_kernel<__half><<<agrid, 128, 0, stream>>>(kc, vc, k_cache.row_stride * 2,
+                                                                   k_cache.head_stride * 2, kn, vn, p, head_dim * 2);
     else if (dtype == kDtypeBF16)
       dec::decode_append_e4m3_kernel<<<agrid, 128, 0, stream>>>(
           kc, vc, k_cache.row_stride, k_cache.head_stride, static_cast<const __nv_bfloat16*>(k_new),

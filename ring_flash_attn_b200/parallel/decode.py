@@ -107,12 +107,16 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
                   v: Optional[Tensor], causal: bool, softmax_scale: float, pg=None, world: int = 1,
                   splits: Optional[int] = None, block_table: Optional[Tensor] = None,
                   k_descale: Optional[Tensor] = None, v_descale: Optional[Tensor] = None,
-                  cu_seqlens_q: Optional[Tensor] = None, max_seqlen_q: Optional[int] = None) -> Tuple[Tensor, Tensor]:
+                  cu_seqlens_q: Optional[Tensor] = None, max_seqlen_q: Optional[int] = None,
+                  rotary_cos: Optional[Tensor] = None, rotary_sin: Optional[Tensor] = None,
+                  rotary_seqlens: Optional[Tensor] = None, rotary_interleaved: bool = True) -> Tuple[Tensor, Tensor]:
     """Local split-KV kernel (appending ``k`` / ``v`` first when given), then the combine over the splits and, for
     ``world > 1``, over the gathered per-rank partials.  ``splits`` overrides :func:`num_splits`.  With
     ``block_table`` the caches are page pools (see :func:`cp_flash_attn_with_kvcache`).  e4m3 caches take contiguous
     fp32 ``(B, Hkv)`` ``k_descale`` / ``v_descale``.  With ``cu_seqlens_q`` (and ``max_seqlen_q``) ``q`` / ``k`` /
-    ``v`` are varlen ``(total_q, H, D)`` and the result is ``out (total_q, Hq, D)``, ``lse (Hq, total_q)``."""
+    ``v`` are varlen ``(total_q, H, D)`` and the result is ``out (total_q, Hq, D)``, ``lse (Hq, total_q)``.  With
+    ``rotary_cos`` / ``rotary_sin`` (and ``rotary_seqlens``, required here) the kernel rotates ``q`` as it loads it
+    and ``k`` before it stores it, as :func:`apply_rotary` does, at positions clamped to the tables."""
     C = cuda_ext.load()
     varlen = cu_seqlens_q is not None
     if varlen:  # the partials are the uniform layout at batch 1, Sq = total_q
@@ -136,7 +140,8 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
     size = n_out + rows_b * hq * rows_sq
     parts = torch.empty((splits, size), dtype=torch.float32, device=q.device)
     C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts, block_table, k_descale,
-                 v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0)
+                 v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0, rotary_cos, rotary_sin, rotary_seqlens,
+                 bool(rotary_interleaved))
     cuda_ext.note_launch(2 if k is not None else 1)
     if world > 1:
         mine = torch.empty(size, dtype=torch.float32, device=q.device)
@@ -160,6 +165,40 @@ def quantize_e4m3(x: Tensor, descale: Tensor) -> Tensor:
     return (x.float() / descale[:, None]).clamp(-448, 448).to(torch.float8_e4m3fn)
 
 
+def apply_rotary(x: Tensor, cos: Tensor, sin: Tensor, positions: Tensor, interleaved: bool = True) -> Tensor:
+    """``x`` ``(..., H, D)`` with rotary embeddings at table rows ``positions`` (shape ``x.shape[:-2]``), from the
+    ``(seqlen_ro, rotary_dim / 2)`` tables ``cos`` / ``sin``.  Columns below ``rotary_dim`` are rotated in pairs
+    ``(i, i + rotary_dim / 2)`` (GPT-NeoX / Llama), or ``(2i, 2i + 1)`` when ``interleaved`` (GPT-J); the rest are left
+    as they are.  For a pair ``(a, b)`` and ``c = cos[pos, i]``, ``s = sin[pos, i]``: ``a' = a c - b s``,
+    ``b' = b c + a s``, with every operand widened to fp32, each product and the sum or difference rounded to fp32
+    (no FMA), and the result rounded to nearest even into x's dtype.  The sm_90a decode kernel computes exactly this,
+    so a fused call is bitwise a plain call on rotated inputs."""
+    h = cos.shape[1]
+    c = cos[positions].float().unsqueeze(-2)  # (..., 1, h)
+    s = sin[positions].float().unsqueeze(-2)
+    xr = x[..., :2 * h].float()
+    a, b = (xr[..., 0::2], xr[..., 1::2]) if interleaved else (xr[..., :h], xr[..., h:])
+    a2 = a * c - b * s  # separate torch ops: each rounded to fp32
+    b2 = b * c + a * s
+    y = torch.stack([a2, b2], dim=-1).flatten(-2) if interleaved else torch.cat([a2, b2], dim=-1)
+    return torch.cat([y.to(x.dtype), x[..., 2 * h:]], dim=-1)
+
+
+def _rotary_positions(rotary_seqlens: Tensor, spans, seqlen_ro: int, causal: bool, device):
+    """Table rows of the packed new tokens, (keys, queries): key t of sequence b at ``rotary_seqlens[b] + t``, query
+    token t there too when causal, at ``rotary_seqlens[b]`` otherwise.  ``ValueError`` for a position outside the
+    tables (the kernel clamps instead)."""
+    keys, queries = [], []
+    for i, (start, (_, n)) in enumerate(zip(rotary_seqlens.tolist(), spans)):
+        if n and not 0 <= start <= seqlen_ro - n:
+            raise ValueError(f"rotary positions [{start}, {start + n}) of sequence {i} are outside the "
+                             f"{seqlen_ro}-row rotary tables")
+        keys += range(start, start + n)
+        queries += range(start, start + n) if causal else [start] * n
+    return (torch.tensor(keys, dtype=torch.long, device=device), torch.tensor(queries, dtype=torch.long,
+                                                                              device=device))
+
+
 def _varlen_spans(cu_seqlens_q: Tensor, total_q: int, max_seqlen_q: int):
     """(first row, count) of every sequence of a varlen call; ``ValueError`` for a malformed ``cu_seqlens_q``."""
     cu = cu_seqlens_q.tolist()
@@ -174,7 +213,7 @@ def _varlen_spans(cu_seqlens_q: Tensor, total_q: int, max_seqlen_q: int):
 
 
 def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table=None,
-                  k_descale=None, v_descale=None, cu_seqlens_q=None, max_seqlen_q=0):
+                  k_descale=None, v_descale=None, cu_seqlens_q=None, max_seqlen_q=0, rotary=None):
     # every sequence is a (first row, count) span of the packed rows: (b * Sq, Sq) for a uniform q
     b = cache_seqlens.shape[0]
     hq, d = q.shape[-2:]
@@ -186,6 +225,12 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
         q = q.reshape(b * sq, hq, d)
         if k is not None:
             k, v = k.reshape(b * sq, *k.shape[2:]), v.reshape(b * sq, *v.shape[2:])
+    if rotary is not None:  # (cos, sin, rotary_seqlens, interleaved): q on every rank, k where it is appended
+        cos, sin, rotary_seqlens, interleaved = rotary
+        key_pos, q_pos = _rotary_positions(rotary_seqlens, spans, cos.shape[0], causal, q.device)
+        q = apply_rotary(q, cos, sin, q_pos, interleaved)
+        if k is not None:
+            k = apply_rotary(k, cos, sin, key_pos, interleaved)
     rows = q.shape[0]
     s_cap = _capacity(k_cache, block_table)
     lens = [max(0, min(int(x), s_cap)) for x in cache_seqlens.tolist()]
@@ -250,12 +295,16 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
 def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor, k: Optional[Tensor],
               v: Optional[Tensor], append_rank: int, softmax_scale: float, causal: bool, group: str,
               block_table: Optional[Tensor], k_descale: Optional[Tensor], v_descale: Optional[Tensor],
-              cu_seqlens_q: Optional[Tensor], max_seqlen_q: int) -> Tuple[Tensor, Tensor]:
+              cu_seqlens_q: Optional[Tensor], max_seqlen_q: int, rotary_cos: Optional[Tensor] = None,
+              rotary_sin: Optional[Tensor] = None, rotary_seqlens: Optional[Tensor] = None,
+              rotary_interleaved: bool = True) -> Tuple[Tensor, Tensor]:
     """q (B, Sq, Hq, D) -> (out (B, Sq, Hq, D) in q.dtype, lse (B, Hq, Sq) fp32).  ``k`` / ``v`` are appended to
     the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's name ("" = world);
     with ``block_table`` the caches are this rank's page pools; e4m3 caches come with contiguous fp32 (B, Hkv)
     ``k_descale`` / ``v_descale``.  With ``cu_seqlens_q`` q / k / v are varlen (total_q, H, D), out is
-    (total_q, Hq, D) and lse (Hq, total_q); ``max_seqlen_q`` bounds the counts (0 when uniform)."""
+    (total_q, Hq, D) and lse (Hq, total_q); ``max_seqlen_q`` bounds the counts (0 when uniform).  With
+    ``rotary_cos`` / ``rotary_sin`` / ``rotary_seqlens``, every rank rotates q and the append rank rotates k before
+    it stores it."""
     pg = resolve_group(group)
     rank, world = group_info(pg)
     if k is not None and not 0 <= append_rank < world:
@@ -265,14 +314,18 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
     if _kernel_takes(q):
         return kernel_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world,
                              block_table=block_table, k_descale=k_descale, v_descale=v_descale,
-                             cu_seqlens_q=cu_seqlens_q, max_seqlen_q=max_seqlen_q)
+                             cu_seqlens_q=cu_seqlens_q, max_seqlen_q=max_seqlen_q, rotary_cos=rotary_cos,
+                             rotary_sin=rotary_sin, rotary_seqlens=rotary_seqlens,
+                             rotary_interleaved=rotary_interleaved)
+    rotary = None if rotary_cos is None else (rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved)
     return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table,
-                         k_descale, v_descale, cu_seqlens_q, max_seqlen_q)
+                         k_descale, v_descale, cu_seqlens_q, max_seqlen_q, rotary)
 
 
 @cp_decode.register_fake
 def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group, block_table, k_descale,
-      v_descale, cu_seqlens_q, max_seqlen_q):
+      v_descale, cu_seqlens_q, max_seqlen_q, rotary_cos=None, rotary_sin=None, rotary_seqlens=None,
+      rotary_interleaved=True):
     if cu_seqlens_q is not None:
         total_q, hq, _ = q.shape
         return q.new_empty(q.shape), q.new_empty((hq, total_q), dtype=torch.float32)
@@ -313,10 +366,44 @@ def _check_descale(name, x, q, b, hkv):
     return x.expand(b, hkv).contiguous()
 
 
+def _check_rotary(cos, sin, rotary_seqlens, q, b, d, cache_seqlens, group):
+    """Checks the rotary tables and returns the (B,) positions the kernels read: ``rotary_seqlens``, or
+    ``cache_seqlens`` in a one-rank group."""
+    if cos is None or sin is None:
+        raise ValueError("pass both rotary_cos and rotary_sin, or neither")
+    for name, x in (("rotary_cos", cos), ("rotary_sin", sin)):
+        if not isinstance(x, Tensor) or x.dim() != 2 or not x.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous (seqlen_ro, rotary_dim / 2) tensor")
+        if x.dtype != q.dtype:
+            raise ValueError(f"{name} must have q's dtype ({q.dtype}), not {x.dtype}")
+        if x.device != q.device:
+            raise ValueError(f"{name} must be on q's device")
+    if cos.shape != sin.shape:
+        raise ValueError(f"rotary_cos {tuple(cos.shape)} and rotary_sin {tuple(sin.shape)} must have the same shape")
+    rotary_dim = 2 * cos.shape[1]
+    if rotary_dim == 0 or rotary_dim % 16 != 0 or rotary_dim > d:
+        raise ValueError(f"rotary_dim = 2 * rotary_cos.shape[1] = {rotary_dim} must be a positive multiple of 16 "
+                         f"and at most head_dim = {d}")
+    if not 1 <= cos.shape[0] < 2 ** 31:
+        raise ValueError(f"rotary_cos must have between 1 and 2^31 - 1 rows, not {cos.shape[0]}")
+    if rotary_seqlens is None:
+        if group_info(resolve_group(group_name(group)))[1] > 1:
+            raise ValueError("rotary_seqlens is required in a group of more than one rank: cache_seqlens are the "
+                             "lengths of this rank's shard, not the positions of the new tokens")
+        return cache_seqlens
+    if (not isinstance(rotary_seqlens, Tensor) or rotary_seqlens.dtype != torch.int32
+            or tuple(rotary_seqlens.shape) != (b,) or not rotary_seqlens.is_contiguous()):
+        raise ValueError(f"rotary_seqlens must be a contiguous (B,) = ({b},) int32 tensor")
+    if rotary_seqlens.device != q.device:
+        raise ValueError("rotary_seqlens must be on q's device")
+    return rotary_seqlens
+
+
 def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=None, append_rank=None,
                                softmax_scale=None, causal=True, return_softmax_lse=False, group=None, *,
                                block_table=None, k_descale=None, v_descale=None, cu_seqlens_q=None,
-                               max_seqlen_q=None, window_size=(-1, -1), alibi_slopes=None):
+                               max_seqlen_q=None, rotary_cos=None, rotary_sin=None, rotary_interleaved=True,
+                               rotary_seqlens=None, window_size=(-1, -1), alibi_slopes=None):
     """Decode attention of new query tokens against a KV cache sharded over ``group`` (modelled on flash-attn's
     ``flash_attn_with_kvcache``).  Inference only: no gradient.
 
@@ -368,9 +455,23 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
     * ``window_size``, ``alibi_slopes``, ``D > 128`` and ``Hq % Hkv != 0`` raise ``ValueError``.  The sm_90a kernel
       covers a bf16 / fp16 ``q`` with ``D`` in {64, 128}, over caches in q's dtype or e4m3; other head sizes run the
       dense torch path with a one-time warning.
-    * Nothing is read back to the host on the kernel path, so a decode step can be captured in a CUDA graph.
-
-    RoPE: the positions of the new tokens are the caller's to apply (prefill length plus the decode step)."""
+    * Rotary embeddings (flash-attn's ``rotary_cos`` / ``rotary_sin`` / ``rotary_interleaved``, and flash-attn 3's
+      ``rotary_seqlens``): ``rotary_cos`` / ``rotary_sin`` are contiguous ``(seqlen_ro, rotary_dim / 2)`` tensors in
+      q's dtype on q's device, the same on every rank; ``rotary_dim`` is a multiple of 16 and at most ``D``, and
+      columns at or past it are left as they are.  ``rotary_interleaved=True`` pairs columns ``(2i, 2i + 1)``
+      (GPT-J), ``False`` pairs ``i`` and ``i + rotary_dim / 2`` (GPT-NeoX / Llama).  ``rotary_seqlens`` ``(B,)``
+      int32 on q's device, the same on every rank, is the global position of each sequence's first new token: new key
+      ``t`` of sequence ``b`` is rotated at ``rotary_seqlens[b] + t``, and query token ``t`` there too when
+      ``causal``, at ``rotary_seqlens[b]`` otherwise (``t`` counts from ``cu_seqlens_q[b]`` in a varlen call).
+      ``cache_seqlens`` are shard lengths, not positions, so ``rotary_seqlens`` is required in a group of more than
+      one rank; in a one-rank group it defaults to ``cache_seqlens`` (flash-attn's rule).  Rotary needs ``k`` /
+      ``v``.  The appended ``k`` is stored rotated (for an e4m3 cache, rotated, rounded to q's dtype, then
+      quantised).  The rotation is :func:`apply_rotary`'s exactly, so a call is bitwise a call without rotary on
+      rotated ``q`` / ``k``.  The kernel path reads ``rotary_seqlens`` on the device only (a CUDA graph replay uses
+      its current contents) and clamps every position to ``[0, seqlen_ro - 1]``; the dense path raises
+      ``ValueError`` for a position outside the tables.  Malformed tables or ``rotary_seqlens`` (one of cos / sin,
+      shapes, dtype, device, ``rotary_dim``) raise ``ValueError``.
+    * Nothing is read back to the host on the kernel path, so a decode step can be captured in a CUDA graph."""
     if tuple(window_size) != (-1, -1):
         raise ValueError("cp_flash_attn_with_kvcache: sliding windows are not supported in decode")
     if alibi_slopes is not None:
@@ -444,8 +545,15 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
                 raise ValueError(f"k / v must be (B, Sq, Hkv, D) = {(b, sq, hkv, d)} in q's dtype")
     elif append_rank is not None:
         raise ValueError("append_rank must be None when no k / v are given")
+    if rotary_cos is not None or rotary_sin is not None:
+        rotary_seqlens = _check_rotary(rotary_cos, rotary_sin, rotary_seqlens, q, b, d, cache_seqlens, group)
+        if k is None:
+            raise ValueError("rotary_cos / rotary_sin need k / v: the rotation applies to the new tokens")
+    elif rotary_seqlens is not None:
+        raise ValueError("rotary_seqlens is only taken with rotary_cos / rotary_sin")
     scale = float(softmax_scale) if softmax_scale is not None else d ** -0.5
     out, lse = cp_decode(q, k_cache, v_cache, cache_seqlens, k, v, -1 if append_rank is None else int(append_rank),
                          scale, bool(causal), group_name(group), block_table, k_descale, v_descale, cu_seqlens_q,
-                         max_seqlen_q if varlen else 0)
+                         max_seqlen_q if varlen else 0, rotary_cos, rotary_sin, rotary_seqlens,
+                         bool(rotary_interleaved))
     return (out, lse) if return_softmax_lse else out
