@@ -464,9 +464,12 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
   }
   TORCH_CHECK(seqlens.scalar_type() == at::kInt && seqlens.is_cuda() && seqlens.is_contiguous() && seqlens.numel() == B,
               "decode_fwd: cache_seqlens must be (B,) int32 on the device");
-  TORCH_CHECK(part.scalar_type() == at::kFloat && part.is_contiguous() && part.dim() == 2 && part.size(0) >= 1 &&
-                  part.size(1) == rows * hq * d + rows * hq,
-              "decode_fwd: part must be fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq), or total_q for B*Sq when varlen");
+  // the kernel stores out as float2: every split's partial must start 8-byte aligned
+  TORCH_CHECK(part.scalar_type() == at::kFloat && part.dim() == 2 && part.size(0) >= 1 && part.stride(1) == 1 &&
+                  part.size(1) == rows * hq * d + rows * hq && part.stride(0) >= part.size(1) &&
+                  part.stride(0) % 2 == 0 && reinterpret_cast<uintptr_t>(part.data_ptr()) % 8 == 0,
+              "decode_fwd: part must be fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq), or total_q for B*Sq when varlen, with "
+              "stride(1) == 1, an even stride(0) and an 8-byte aligned start");
   TORCH_CHECK(k_new.has_value() == v_new.has_value(), "decode_fwd: pass both k_new and v_new or neither");
   const void* kn = nullptr;
   const void* vn = nullptr;
@@ -490,7 +493,7 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
   p.q_head_stride = q.stride(2);
   p.seqlens = seqlens.data_ptr<int>();
   p.part = part.data_ptr<float>();
-  p.part_stride = part.size(1);
+  p.part_stride = part.stride(0);
   p.batch = static_cast<int>(B);
   p.sq = static_cast<int>(sq);
   p.hq = static_cast<int>(hq);
@@ -552,13 +555,13 @@ void decode_combine(const at::Tensor& parts, at::Tensor& out, at::Tensor& lse) {
   const c10::cuda::CUDAGuard guard(parts.device());
   TORCH_CHECK(out.dim() == 4 && out.is_contiguous() && out.is_cuda(), "decode_combine: out must be contiguous (B, Sq, Hq, D)");
   const int64_t B = out.size(0), sq = out.size(1), hq = out.size(2), d = out.size(3);
-  TORCH_CHECK(parts.scalar_type() == at::kFloat && parts.is_contiguous() && parts.dim() == 2 && parts.size(0) >= 1 &&
-                  parts.size(1) == B * sq * hq * d + B * hq * sq,
-              "decode_combine: parts must be fp32 (P, B*Sq*Hq*D + B*Hq*Sq)");
+  TORCH_CHECK(parts.scalar_type() == at::kFloat && parts.dim() == 2 && parts.size(0) >= 1 && parts.stride(1) == 1 &&
+                  parts.stride(0) >= parts.size(1) && parts.size(1) == B * sq * hq * d + B * hq * sq,
+              "decode_combine: parts must be fp32 (P, B*Sq*Hq*D + B*Hq*Sq) with stride(1) == 1");
   TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == B * hq * sq,
               "decode_combine: lse must be fp32 (B, Hq, Sq)");
   const int out_dtype = out.scalar_type() == at::kFloat ? -1 : dtype_code(out);
-  check(rfa::decode_combine_launch(parts.data_ptr<float>(), parts.size(1), static_cast<int>(parts.size(0)),
+  check(rfa::decode_combine_launch(parts.data_ptr<float>(), parts.stride(0), static_cast<int>(parts.size(0)),
                                    static_cast<int>(B), static_cast<int>(sq), static_cast<int>(hq), static_cast<int>(d),
                                    out.data_ptr(), out_dtype, lse.data_ptr<float>(), at::cuda::getCurrentCUDAStream()));
 }

@@ -8,7 +8,8 @@
 namespace rfa {
 
 // Partial results live in one fp32 buffer per split (or per rank): the (b, t, h) rows of `out` (rows x head_dim),
-// followed by `lse` in the (b, h, t) order of the public softmax_lse.  part_stride = elements per split.  A varlen
+// followed by `lse` in the (b, h, t) order of the public softmax_lse.  part_stride = elements from one split's
+// partial to the next, even for decode_kernel (it stores out as float2), so it may exceed the partial's size.  A varlen
 // call (cu_seqlens_q set) uses the same layout at batch 1, sq = total_q: out rows (cu[b] + t, h), lse (h, cu[b] + t).
 struct DecodeParams {
   const void* q;           // (B * Sq, Hq, D) view of (B, Sq, Hq, D), or varlen (total_q, Hq, D)

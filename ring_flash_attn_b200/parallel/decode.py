@@ -138,7 +138,9 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
             splits = num_splits(b, sq, hq, hkv, s_cap, _sm_count(dev))
     n_out = rows_b * rows_sq * hq * d
     size = n_out + rows_b * hq * rows_sq
-    parts = torch.empty((splits, size), dtype=torch.float32, device=q.device)
+    # every split's partial starts 8-byte aligned (the kernel stores out as float2): rows * Hq * (D + 1) is odd when
+    # rows and Hq are
+    parts = torch.empty((splits, size + size % 2), dtype=torch.float32, device=q.device)[:, :size]
     C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts, block_table, k_descale,
                  v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0, rotary_cos, rotary_sin, rotary_seqlens,
                  bool(rotary_interleaved))
