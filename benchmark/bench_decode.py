@@ -11,6 +11,10 @@ With ``--kv-dtype e4m3`` every configuration also times the kernel over an e4m3 
 per-(sequence, kv head) descales; paged too with ``--page-size``) in the same loop, and reports its bytes, rate,
 speed-up over the bf16 kernel, whether its output at unit descales is bitwise the bf16 kernel's on the widened cache,
 and its largest difference from the bf16 output (the quantisation error, for information).
+With ``--q-dtype e4m3`` (which needs ``--kv-dtype e4m3``) the loop gains a third arm: the fp8-query kernel (an e4m3
+query with per-(sequence, kv head) ``q_descale``, Q K^T as an e4m3 wgmma) over the same e4m3 cache (paged too with
+``--page-size``); the line reports its time, its speed-up over the bf16 arm and over the bf16-query e4m3-cache arm,
+and its largest difference from the bf16 output (for information).
 With ``--mixed-chunk C`` every configuration also times, in the same loop, a varlen call (``cu_seqlens_q``) where
 sequence 0 brings C new tokens and the others 1, the uniform call padded to Sq = C (what a caller without varlen
 must do) and the uniform Sq = 1 call (the pure-decode floor), with the K + V bytes the varlen and padded calls stream
@@ -23,6 +27,7 @@ plain call alone; and reports whether the fused and unfused outputs are bitwise 
     python benchmark/bench_decode.py                      # B in {1, 8}, caches of 32K..512K tokens per rank
     python benchmark/bench_decode.py --page-size 16       # also the paged kernel, pages of 16 rows
     python benchmark/bench_decode.py --kv-dtype e4m3      # also the fp8-cache kernel
+    python benchmark/bench_decode.py --kv-dtype e4m3 --q-dtype e4m3   # and the fp8-query kernel
     python benchmark/bench_decode.py --mixed-chunk 64     # also a ragged batch: one 64-token chunk + decodes
     python benchmark/bench_decode.py --rotary             # also the fused RoPE step against the unfused one
     torchrun --nproc-per-node 2 benchmark/bench_decode.py
@@ -57,13 +62,21 @@ def parse_args(argv=None):
     ap.add_argument("--page-size", type=int, default=None, help="also time a paged cache with pages of N rows")
     ap.add_argument("--kv-dtype", choices=("bf16", "e4m3"), default="bf16",
                     help="e4m3: also time an fp8 (e4m3) cache with per-head descales")
+    ap.add_argument("--q-dtype", choices=("bf16", "e4m3"), default="bf16",
+                    help="e4m3: also time fp8 (e4m3) queries over the e4m3 cache (needs --kv-dtype e4m3)")
     ap.add_argument("--mixed-chunk", type=int, default=None, metavar="C",
                     help="also time a varlen batch (sequence 0 brings C tokens, the others 1) against the uniform "
                          "call padded to Sq = C and the uniform Sq = 1 call")
     ap.add_argument("--rotary", action="store_true",
                     help="also time a RoPE step: the fused call, the torch rotation + a plain call, the plain call")
     ap.add_argument("--dry-run", action="store_true")
-    return ap.parse_args(argv)
+    args = ap.parse_args(argv)
+    if args.q_dtype == "e4m3" and args.kv_dtype != "e4m3":
+        ap.error("--q-dtype e4m3 needs --kv-dtype e4m3 (fp8 queries run over e4m3 caches only)")
+    return args
+
+
+Q8_FIELDS = ["q8_us", "q8_speedup_vs_bf16", "q8_speedup_vs_fp8", "q8_max_abs_diff_vs_bf16"]
 
 
 def shapes(args, sm_count):
@@ -77,6 +90,8 @@ def shapes(args, sm_count):
                 cfg.update(page_size=args.page_size, block_table_bytes=b * -(-s // args.page_size) * 4)
             if args.kv_dtype == "e4m3":  # one byte per cached element
                 cfg.update(kv_dtype="e4m3", fp8_kv_bytes=cfg["kv_bytes"] // 2)
+            if args.q_dtype == "e4m3":  # the fields the timed run adds
+                cfg.update(q_dtype="e4m3", q8_fields=Q8_FIELDS)
             if args.mixed_chunk:
                 c, g = args.mixed_chunk, args.hq // args.hkv
                 total_q = c + b - 1
@@ -166,6 +181,19 @@ def main():
             del wk, wv, unit, wide
             fp8_res["fp8_max_abs_diff_vs_bf16"] = (ours_fp8()[0].float() - ours()[0].float()).abs().max().item()
 
+        q8 = args.q_dtype == "e4m3"
+        if q8:  # e4m3 queries with per-(sequence, kv head) descales amax / 448, over the same e4m3 cache
+            g = args.hq // args.hkv
+            qd = q.float().view(b, args.sq, args.hkv, g, d).abs().amax(dim=(1, 3, 4)).clamp(min=1e-12) / 448
+            q_e4m3 = (q.float() / qd.repeat_interleave(g, dim=1)[:, None, :, None]).clamp(-448, 448).to(
+                torch.float8_e4m3fn)
+
+            def ours_q8():
+                return dec.kernel_decode(q_e4m3, k8, v8, sl, None, None, True, scale, k_descale=kd, v_descale=vd,
+                                         q_descale=qd)
+
+            fp8_res["q8_max_abs_diff_vs_bf16"] = (ours_q8()[0].float() - ours()[0].float()).abs().max().item()
+
         if args.page_size:  # the same rows in a pool whose pages are in a seeded random order
             ps = args.page_size
             max_blocks = -(-s // ps)
@@ -190,6 +218,10 @@ def main():
                 def paged_fp8():
                     return dec.kernel_decode(q, p8k, p8v, sl, None, None, True, scale, block_table=table,
                                              k_descale=kd, v_descale=vd)
+
+                def paged_q8():
+                    return dec.kernel_decode(q_e4m3, p8k, p8v, sl, None, None, True, scale, block_table=table,
+                                             k_descale=kd, v_descale=vd, q_descale=qd)
 
         if args.mixed_chunk:  # sequence 0 brings C new tokens, the others 1, over the same caches
             c = args.mixed_chunk
@@ -243,6 +275,10 @@ def main():
             rows["fp8"] = []
             if args.page_size:
                 rows["paged_fp8"] = []
+        if q8:
+            rows["q8"] = []
+            if args.page_size:
+                rows["paged_q8"] = []
         mixed_rows = {"mixed_varlen": [], "mixed_padded": [], "mixed_decode_only": []}
         rot_rows = {"rotary_fused": [], "rotary_unfused": [], "rotary_plain": []}
         sdpa_err = None
@@ -262,6 +298,10 @@ def main():
                 rows["fp8"].append(time_us(ours_fp8, args.iters, args.warmup))
                 if args.page_size:
                     rows["paged_fp8"].append(time_us(paged_fp8, args.iters, args.warmup))
+            if q8:
+                rows["q8"].append(time_us(ours_q8, args.iters, args.warmup))
+                if args.page_size:
+                    rows["paged_q8"].append(time_us(paged_q8, args.iters, args.warmup))
             if sdpa_err is None:
                 try:
                     rows["sdpa"].append(time_us(sdpa, args.iters, args.warmup))
@@ -272,7 +312,7 @@ def main():
         for k, ts in rows.items():
             if ts:
                 us = min(ts)
-                nbytes = cfg["fp8_kv_bytes"] if k.endswith("fp8") else cfg["kv_bytes"]
+                nbytes = cfg["fp8_kv_bytes"] if k.endswith(("fp8", "q8")) else cfg["kv_bytes"]
                 res[f"{k}_us"] = round(us, 2)
                 res[f"{k}_us_all"] = [round(t, 2) for t in ts]
                 res[f"{k}_GBps"] = round(nbytes / (us * 1e-6) / 1e9, 1)
@@ -302,6 +342,13 @@ def main():
             if args.page_size:
                 res["paged_fp8_speedup_vs_paged"] = round(res["paged_us"] / res["paged_fp8_us"], 3)
                 res["paged_fp8_equal_contiguous_fp8"] = all(torch.equal(x, y) for x, y in zip(paged_fp8(), ours_fp8()))
+            if q8:
+                res["q8_speedup_vs_bf16"] = round(res["ours_us"] / res["q8_us"], 3)
+                res["q8_speedup_vs_fp8"] = round(res["fp8_us"] / res["q8_us"], 3)
+                if args.page_size:
+                    res["paged_q8_speedup_vs_paged"] = round(res["paged_us"] / res["paged_q8_us"], 3)
+                    res["paged_q8_speedup_vs_paged_fp8"] = round(res["paged_fp8_us"] / res["paged_q8_us"], 3)
+                    res["paged_q8_equal_contiguous_q8"] = all(torch.equal(x, y) for x, y in zip(paged_q8(), ours_q8()))
             res.update(fp8_res)
         if world > 1:
             C = dec.cuda_ext.load()
@@ -328,6 +375,8 @@ def main():
             del pk, pv
         if fp8:
             del k8, v8
+            if q8:
+                del q_e4m3
             if args.page_size:
                 del p8k, p8v
         torch.cuda.empty_cache()

@@ -406,14 +406,17 @@ at::Tensor lse_unflatten(const at::Tensor& lse, const at::Tensor& cu, int64_t ma
 // (B + 1,) int32 (B = seqlens.numel()), q is varlen (total_q, Hq, D), k_new / v_new (total_q, Hkv, D), part fp32
 // (n_splits, total_q*Hq*D + Hq*total_q), and max_seqlen_q >= 1 bounds every count; cu_seqlens_q is not validated.
 // With rotary_cos / rotary_sin (seqlen_ro, rotary_dim / 2) contiguous in q's dtype and rotary_seqlens (B,) int32,
-// q and the appended k are rotated (see DecodeParams); rotary_seqlens is read on the device only.
+// q and the appended k are rotated (see DecodeParams); rotary_seqlens is read on the device only.  q may be
+// float8_e4m3fn over e4m3 caches, with q_descale fp32 (B, Hkv) contiguous on q's device (partials of a bf16 P V);
+// k_new / v_new may be float8_e4m3fn over e4m3 caches (stored as they are), or bf16 / fp16 with an e4m3 q.
 void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
                 const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
                 double scale, at::Tensor& part, const c10::optional<at::Tensor>& block_table,
                 const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale,
                 const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q,
                 const c10::optional<at::Tensor>& rotary_cos, const c10::optional<at::Tensor>& rotary_sin,
-                const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved) {
+                const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved,
+                const c10::optional<at::Tensor>& q_descale) {
   const c10::cuda::CUDAGuard guard(q_in.device());
   const bool varlen = cu_seqlens_q.has_value();
   TORCH_CHECK(q_in.dim() == (varlen ? 3 : 4), "decode_fwd: q must be (B, Sq, Hq, D), or (total_q, Hq, D) with "
@@ -431,10 +434,13 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
   TORCH_CHECK(k_cache.dim() == 4 && v_cache.dim() == 4, "decode_fwd: 4-D k_cache / v_cache");
   TORCH_CHECK(k_cache.sizes() == v_cache.sizes(), "decode_fwd: k_cache and v_cache shapes differ");
   const bool fp8 = k_cache.scalar_type() == at::kFloat8_e4m3fn;
+  const bool q8 = q.scalar_type() == at::kFloat8_e4m3fn;
   TORCH_CHECK(k_cache.scalar_type() == v_cache.scalar_type() && (fp8 || k_cache.scalar_type() == q.scalar_type()),
               "decode_fwd: caches must both have q's dtype or both be fp8 (float8_e4m3fn)");
+  TORCH_CHECK(!q8 || fp8, "decode_fwd: an fp8 (float8_e4m3fn) q needs fp8 caches");
   TORCH_CHECK(k_descale.has_value() == fp8 && v_descale.has_value() == fp8,
               "decode_fwd: fp8 caches need k_descale and v_descale, and other caches take none");
+  TORCH_CHECK(q_descale.has_value() == q8, "decode_fwd: an fp8 q needs q_descale, and other queries take none");
   const int64_t B = varlen ? seqlens.numel() : q.size(0);
   const int64_t sq = varlen ? max_seqlen_q : q.size(1), hq = q.size(2), d = q.size(3);
   const int64_t rows = varlen ? total_q : B * sq;  // packed query rows
@@ -446,7 +452,7 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
   TORCH_CHECK((paged || k_cache.size(0) == B) && k_cache.size(3) == d, "decode_fwd: cache shape does not match q");
   TORCH_CHECK(q.stride(3) == 1 && (varlen || q.stride(0) == sq * q.stride(1)),
               "decode_fwd: q must be (B, Sq) mergeable");
-  TORCH_CHECK((q.stride(1) * 2) % 16 == 0 && (q.stride(2) * 2) % 16 == 0 &&
+  TORCH_CHECK((q.stride(1) * q.element_size()) % 16 == 0 && (q.stride(2) * q.element_size()) % 16 == 0 &&
                   reinterpret_cast<uintptr_t>(q.data_ptr()) % 16 == 0,
               "decode_fwd: q rows must be 16-byte aligned");
   for (const at::Tensor* c : {&k_cache, &v_cache})
@@ -473,15 +479,21 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
   TORCH_CHECK(k_new.has_value() == v_new.has_value(), "decode_fwd: pass both k_new and v_new or neither");
   const void* kn = nullptr;
   const void* vn = nullptr;
+  int new_dtype = q8 ? rfa::kDtypeE4M3 : dtype_code(q);
   if (k_new.has_value()) {
+    // q's dtype; e4m3 over an e4m3 cache (stored as they are); bf16 / fp16 with an e4m3 q (quantised)
+    const at::ScalarType nt = k_new->scalar_type();
+    const bool nt_ok = nt == q.scalar_type() || (fp8 && nt == at::kFloat8_e4m3fn) ||
+                       (q8 && (nt == at::kBFloat16 || nt == at::kHalf));
     for (const at::Tensor* t : {&*k_new, &*v_new}) {
       const bool shape_ok = varlen ? t->dim() == 3 && t->size(0) == total_q && t->size(1) == hkv && t->size(2) == d
                                    : t->dim() == 4 && t->size(0) == B && t->size(1) == sq && t->size(2) == hkv &&
                                          t->size(3) == d;
-      TORCH_CHECK(t->is_contiguous() && t->scalar_type() == q.scalar_type() && shape_ok,
+      TORCH_CHECK(t->is_contiguous() && t->scalar_type() == nt && nt_ok && shape_ok,
                   "decode_fwd: k_new / v_new must be contiguous (B, Sq, Hkv, D), or varlen (total_q, Hkv, D), in "
-                  "q's dtype");
+                  "q's dtype, or both e4m3 over e4m3 caches, or bf16 / fp16 with an e4m3 q");
     }
+    new_dtype = nt == at::kFloat8_e4m3fn ? rfa::kDtypeE4M3 : dtype_code(*k_new);
     kn = k_new->data_ptr();
     vn = v_new->data_ptr();
   }
@@ -519,9 +531,18 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
     p.k_descale = k_descale->data_ptr<float>();
     p.v_descale = v_descale->data_ptr<float>();
   }
+  if (q8) {
+    const at::Tensor& t = *q_descale;
+    TORCH_CHECK(t.scalar_type() == at::kFloat && t.is_cuda() && t.device() == q.device() && t.dim() == 2 &&
+                    t.size(0) == B && t.size(1) == hkv && t.is_contiguous(),
+                "decode_fwd: q_descale must be contiguous fp32 (B, Hkv) on q's device");
+    p.q_descale = t.data_ptr<float>();
+  }
   TORCH_CHECK(rotary_cos.has_value() == rotary_sin.has_value() && rotary_cos.has_value() == rotary_seqlens.has_value(),
               "decode_fwd: rotary needs rotary_cos, rotary_sin and rotary_seqlens together");
   if (rotary_cos.has_value()) {
+    TORCH_CHECK(!q8 && new_dtype != rfa::kDtypeE4M3,
+                "decode_fwd: rotary needs a bf16 / fp16 q and k_new (rotate before quantising)");
     const at::Tensor& rc = *rotary_cos;
     const at::Tensor& rs = *rotary_sin;
     TORCH_CHECK(rc.dim() == 2 && rc.sizes() == rs.sizes() && rc.size(0) >= 1 && rc.is_contiguous() &&
@@ -545,8 +566,9 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
   }
   const TensorView kv{k_cache.data_ptr(), cache_rows, static_cast<int>(hkv), k_cache.stride(1), k_cache.stride(2)};
   const TensorView vv{v_cache.data_ptr(), cache_rows, static_cast<int>(hkv), v_cache.stride(1), v_cache.stride(2)};
-  check(rfa::decode_fwd_launch(dtype_code(q), fp8 ? rfa::kDtypeE4M3 : dtype_code(q), kv, vv, kn, vn, p,
-                               static_cast<int>(n_splits), static_cast<int>(d), at::cuda::getCurrentCUDAStream()));
+  check(rfa::decode_fwd_launch(q8 ? rfa::kDtypeE4M3 : dtype_code(q), fp8 ? rfa::kDtypeE4M3 : dtype_code(q), kv, vv,
+                               kn, vn, new_dtype, p, static_cast<int>(n_splits), static_cast<int>(d),
+                               at::cuda::getCurrentCUDAStream()));
 }
 
 // Merges the partials of decode_fwd (or gathered per-rank partials, same layout): out (B, Sq, Hq, D) contiguous in
@@ -614,6 +636,17 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("lse_flatten", &lse_flatten);
   m.def("lse_unflatten", &lse_unflatten);
   m.def("decode_fwd", &decode_fwd);
+  // the same without q_descale (a bf16 / fp16 q)
+  m.def("decode_fwd", [](const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
+                         const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
+                         double scale, at::Tensor& part, const c10::optional<at::Tensor>& block_table,
+                         const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale,
+                         const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q,
+                         const c10::optional<at::Tensor>& rotary_cos, const c10::optional<at::Tensor>& rotary_sin,
+                         const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved) {
+    decode_fwd(q, k_cache, v_cache, seqlens, k_new, v_new, causal, scale, part, block_table, k_descale, v_descale,
+               cu_seqlens_q, max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, c10::nullopt);
+  });
   m.def("decode_combine", &decode_combine);
   rfa::bind_peer_mem(m);
 }

@@ -48,6 +48,8 @@ struct DecodeParams {
   int rotary_half;            // rotary_dim / 2, a multiple of 8
   int seqlen_ro;
   int rotary_interleaved;
+  // e4m3 queries (only over e4m3 caches): q holds x / q_descale[b, kv head]; nullptr for a bf16 / fp16 q
+  const float* q_descale;  // (B, Hkv) contiguous; read on the device only
 };
 
 // Appends k_new / v_new (B, Sq, Hkv, D), contiguous, in q's dtype, at rows [seqlens[b], seqlens[b] + Sq) of the
@@ -57,9 +59,12 @@ struct DecodeParams {
 // are (total_q, Hkv, D) and sequence b's n_b rows go to [seqlens[b], seqlens[b] + n_b); the grid is
 // (n_splits, decode_tile_slots(p), Hkv), each slot mapped to a (sequence, row tile) on the device.  With
 // p.rotary_cos set, q is rotated as the kernel loads it and k_new before it is stored (see DecodeParams).
+// dtype is q's: kDtypeE4M3 (with p.q_descale) only over an e4m3 cache, where S = Q K^T is an e4m3 wgmma on the fp8
+// K tile and the partials are those of a bf16 P V.  new_dtype is k_new / v_new's: q's, or kDtypeE4M3 over an e4m3
+// cache (the bytes are stored as they are), or bf16 / fp16 with an e4m3 q.
 const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_cache, const TensorView& v_cache,
-                              const void* k_new, const void* v_new, const DecodeParams& p, int n_splits, int head_dim,
-                              cudaStream_t stream);
+                              const void* k_new, const void* v_new, int new_dtype, const DecodeParams& p,
+                              int n_splits, int head_dim, cudaStream_t stream);
 
 // Varlen row-tile slots, from shapes only: min(B * ceil(sq * G / 64), (total_q * G + 63 * B) / 64), an upper bound
 // on sum_b ceil(n_b * G / 64) for any counts n_b <= sq that sum to total_q.

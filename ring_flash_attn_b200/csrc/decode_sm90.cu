@@ -16,6 +16,16 @@
 // multiplies its scale_log2 once and v_descale[b, kv head] its 1 / l.  So with power-of-two descales 2^a, 2^c the
 // result is bitwise the bf16 / fp16 kernel's on the widened cache with softmax_scale * 2^a, out scaled by 2^c.
 //
+// e4m3 queries (kQ8, over e4m3 caches only; 288 threads): wgmma takes 8-bit operands K-major, and the e4m3 K tile TMA
+// writes is already K-major for Q K^T, so S = Q K^T is an m64n128k32 e4m3 wgmma with A = the e4m3 Q tile (kD-byte
+// rows in the swizzle of the K tile: 128-byte at kD = 128, 64-byte at 64) and B = the fp8 K slot as TMA filled it.
+// Only V (MN-major in P V) is widened.  The fp8 ring still alternates K, V, K, V (the producer is unchanged); with
+// an even slot count K always lands in even slots, which the compute warps release once the S wgmma has completed,
+// and V in odd ones, which the converter widens into a bf16 ring of V slots only and releases.  Both kinds keep four
+// arrivals per f8_empty.  q_descale[b, kv head] joins k_descale in t2 = scale_log2 * q_descale * k_descale; P and
+// V are bf16 and the rest of the softmax is unchanged.  Shared memory at kD = 128: Q 8 KB + 6 fp8 slots of 16 KB
+// + 3 bf16 V slots of 32 KB + barriers = 206848 bytes with the slack (half of each at kD = 64: 104448).
+//
 // Varlen queries (cu_seqlens_q): sequence b brings n_b = cu[b + 1] - cu[b] tokens.  The grid is (split, tile slot,
 // kv head) instead, with decode_tile_slots() slots, a bound from shapes on sum_b ceil(n_b * G / 64); each CTA finds
 // its (sequence, row tile) by a warp-wide prefix sum over cu, and slots past the last real tile exit at once.
@@ -46,29 +56,38 @@ constexpr int kRows = 64;     // packed query rows per CTA (one wgmma M)
 constexpr int kStages = 6;    // K/V ring slots (one key tile takes two: K, then V)
 constexpr int kStagesFp8 = 4;  // the same with an e4m3 cache, whose kF8Stages fp8 slots take the rest of the memory
 constexpr int kF8Stages = 4;
+constexpr int kF8StagesQ8 = 6;  // e4m3 queries: fp8 K / V slots (even: K in the even slots, V in the odd ones)
+constexpr int kVStagesQ8 = 3;   // e4m3 queries: bf16 slots, V only
+static_assert(kF8StagesQ8 % 2 == 0, "K and V must keep their slot parity");
 constexpr int kThreads = 160;  // one compute warpgroup + one producer warp
 constexpr int kThreadsFp8 = 288;  // + one converter warpgroup
 constexpr int kKHalfBytes = kTile * 128;  // one 64-element-wide (128-byte) swizzled K / V sub-tile
 constexpr int kQHalfBytes = kRows * 128;  // the same for the query tile
 
-template <int kD, bool kFp8>
+template <int kD, bool kFp8, bool kQ8>
 constexpr int smem_bytes() {
+  if constexpr (kQ8)
+    return kRows * kD + kF8StagesQ8 * kTile * kD + kVStagesQ8 * kTile * kD * 2 + 1024 /*barriers*/ +
+           1024 /*align slack*/;
   return kRows * kD * 2 + (kFp8 ? kStagesFp8 * kTile * kD * 3 : kStages * kTile * kD * 2) + 1024 /*barriers*/ +
          1024 /*align slack*/;
 }
 
-struct Barriers {
-  uint64_t kv_full[kStages];
-  uint64_t kv_empty[kStages];
-  uint64_t f8_full[kF8Stages];  // e4m3 caches: the fp8 slots
-  uint64_t f8_empty[kF8Stages];
+template <int kWide, int kLoad>
+struct RingBarriers {
+  uint64_t kv_full[kWide];  // the bf16 / fp16 slots the compute warpgroup reads (V only with e4m3 queries)
+  uint64_t kv_empty[kWide];
+  uint64_t f8_full[kLoad];  // e4m3 caches: the fp8 slots
+  uint64_t f8_empty[kLoad];
 };
+template <bool kQ8>
+using Barriers = std::conditional_t<kQ8, RingBarriers<kVStagesQ8, kF8StagesQ8>, RingBarriers<kStages, kF8Stages>>;
 
 // The ring the TMA producer fills: bf16 / fp16 slots of kD / 64 128-byte-swizzled sub-tiles of 128-byte rows, or
 // e4m3 slots of one sub-tile of kD-byte rows (128-byte swizzle at kD = 128, 64-byte at kD = 64).
-template <int kD, bool kFp8>
+template <int kD, bool kFp8, bool kQ8>
 struct LoadRing {
-  static constexpr int kSlots = kFp8 ? kF8Stages : kStages;
+  static constexpr int kSlots = kQ8 ? kF8StagesQ8 : (kFp8 ? kF8Stages : kStages);
   static constexpr int kSubTiles = kFp8 ? 1 : kD / 64;
   static constexpr int kRowBytes = kFp8 ? kD : 128;  // bytes per row of one sub-tile
   static constexpr int kSlotBytes = kTile * kSubTiles * kRowBytes;
@@ -190,11 +209,11 @@ __device__ __forceinline__ bool varlen_tile(const DecodeParams& p, int slot, int
 // Table entries are read 32 at a time, one per lane, a window ahead of use, and broadcast with shuffles.  The e4m3
 // ring works the same way: a box of page_size < 128 rows is page_size * kD bytes, a multiple of 1024, so every box
 // starts on a swizzle period of the fp8 layout too.
-template <int kD, bool kFp8>
+template <int kD, bool kFp8, bool kQ8>
 __device__ __forceinline__ void produce_paged(const CUtensorMap* tm_k, const CUtensorMap* tm_v, uint64_t* full,
                                               uint64_t* empty, uint8_t* smem_kv, const DecodeParams& p, int b,
                                               int kv_head, int j0, int n_tiles, int kmax) {
-  using L = LoadRing<kD, kFp8>;
+  using L = LoadRing<kD, kFp8, kQ8>;
   constexpr int kSubTiles = L::kSubTiles;
   constexpr int kSlotBytes = L::kSlotBytes;
   const int lane = threadIdx.x & 31;
@@ -281,15 +300,26 @@ __device__ __forceinline__ void widen_tile(const uint8_t* src, uint8_t* dst, int
   }
 }
 
-template <typename T, int kD, bool kFp8>
+// wgmma descriptor of an e4m3 K-major tile of kD-byte rows as TMA writes it (128-byte swizzle at kD = 128, 64-byte
+// at kD = 64); a K step of 32 elements advances the start by 32 bytes.
+template <int kD>
+__device__ __forceinline__ uint64_t f8_desc(const uint8_t* tile) {
+  return kD == 128 ? gmma_desc(smem_u32(tile), 0) : gmma_desc_sw64(smem_u32(tile));
+}
+
+// kQ8: e4m3 queries (T = bf16, kFp8 set), see the file comment.
+template <typename T, int kD, bool kFp8, bool kQ8>
 __global__ void __launch_bounds__(kFp8 ? kThreadsFp8 : kThreads, 1)
 decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
               const __grid_constant__ DecodeParams p) {
   static_assert(kD == 64 || kD == 128, "head dim 64 or 128");
-  using L = LoadRing<kD, kFp8>;
+  static_assert(!kQ8 || (kFp8 && std::is_same_v<T, __nv_bfloat16>), "e4m3 queries: e4m3 cache, bf16 P V");
+  using L = LoadRing<kD, kFp8, kQ8>;
   constexpr int kSubTiles = kD / 64;
-  constexpr int kSlots = kFp8 ? kStagesFp8 : kStages;  // T slots the compute warpgroup reads
+  // T slots the compute warpgroup reads
+  constexpr int kSlots = kQ8 ? kVStagesQ8 : (kFp8 ? kStagesFp8 : kStages);
   constexpr int kSlotBytes = kTile * kD * 2;
+  constexpr int kQBytes = kRows * kD * (kQ8 ? 1 : 2);
   constexpr int kProducer = kFp8 ? 256 : 128;  // first thread of the producer warp
   const int split = blockIdx.x;
   const int group = p.hq / p.hkv;
@@ -320,9 +350,9 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_q = smem;
-  uint8_t* smem_kv = smem + kRows * kD * 2;
+  uint8_t* smem_kv = smem + kQBytes;
   uint8_t* smem_f8 = smem_kv + kSlots * kSlotBytes;  // e4m3 caches only
-  Barriers* bars = reinterpret_cast<Barriers*>(smem_f8 + (kFp8 ? L::kSlots * L::kSlotBytes : 0));
+  auto* bars = reinterpret_cast<Barriers<kQ8>*>(smem_f8 + (kFp8 ? L::kSlots * L::kSlotBytes : 0));
   // the ring TMA fills
   uint8_t* smem_load = kFp8 ? smem_f8 : smem_kv;
   uint64_t* load_full = kFp8 ? bars->f8_full : bars->kv_full;
@@ -336,7 +366,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
       mbar_init(&bars->kv_empty[i], 4);  // one arrival per compute warp
     }
     if constexpr (kFp8) {
-      for (int i = 0; i < kF8Stages; ++i) {
+      for (int i = 0; i < L::kSlots; ++i) {
         mbar_init(&bars->f8_full[i], 1);
         mbar_init(&bars->f8_empty[i], 4);  // one arrival per converter warp
       }
@@ -349,7 +379,8 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
     // ------------------------------------------------------------------ TMA producer
     if (p.page_size != 0) {
       if (n_tiles > 0)
-        produce_paged<kD, kFp8>(&tm_k, &tm_v, load_full, load_empty, smem_load, p, b, kv_head, j0, n_tiles, kmax);
+        produce_paged<kD, kFp8, kQ8>(&tm_k, &tm_v, load_full, load_empty, smem_load, p, b, kv_head, j0, n_tiles,
+                                     kmax);
     } else if (threadIdx.x == kProducer) {
       uint32_t slot = 0, phase = 0;
       for (int jj = 0; jj < n_tiles; ++jj) {
@@ -371,7 +402,33 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
     return;
   }
 
-  if constexpr (kFp8) {
+  if constexpr (kQ8) {
+    if (threadIdx.x >= 128) {
+      // ---------------------------------------------------------------- converter: fp8 V slot -> bf16 V slot
+      uint32_t slot = 0, phase = 0, fslot = 1, fphase = 0;  // V of tile jj is fp8 item 2 jj + 1
+      for (int jj = 0; jj < n_tiles; ++jj) {
+        mbar_wait(&bars->f8_full[fslot], fphase);
+        mbar_wait(&bars->kv_empty[slot], phase ^ 1);
+        widen_tile<T, kD>(smem_f8 + fslot * L::kSlotBytes, smem_kv + slot * kSlotBytes, threadIdx.x - 128);
+        fence_proxy_async_smem();  // the generic-proxy writes, before wgmma reads them
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) {
+          mbar_arrive(&bars->kv_full[slot]);
+          mbar_arrive(&bars->f8_empty[fslot]);
+        }
+        if (++slot == kSlots) {
+          slot = 0;
+          phase ^= 1;
+        }
+        fslot += 2;
+        if (fslot >= L::kSlots) {
+          fslot -= L::kSlots;
+          fphase ^= 1;
+        }
+      }
+      return;
+    }
+  } else if constexpr (kFp8) {
     if (threadIdx.x >= 128) {
       // ---------------------------------------------------------------- converter: fp8 slot -> T slot
       uint32_t slot = 0, phase = 0, fslot = 0, fphase = 0;
@@ -408,20 +465,39 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
 
   // Q tile: packed rows in the 128-byte swizzled K-major layout TMA would write; rows past the group are zero.  With
   // rotary, chunks below rotary_dim are rotated on the way (token t's position; the first token's when not causal).
-  constexpr int kChunks = kD / 8;  // 16-byte chunks per row
+  if constexpr (kQ8) {
+    // e4m3 Q tile: kD-byte rows in the swizzle TMA writes for the e4m3 K tile (no rotary: the caller quantised q)
+    const uint8_t* q8 = static_cast<const uint8_t*>(p.q);
+    constexpr int kChunks = kD / 16;
 #pragma unroll 4
-  for (int idx = tid; idx < kRows * kChunks; idx += 128) {
-    const int r = idx / kChunks, c = idx % kChunks;
-    uint4 val = make_uint4(0u, 0u, 0u, 0u);
-    if (r < rows_here) {
-      const int pr = row0 + r;
-      const int t = pr / group, head = kv_head * group + pr % group;
-      const T* q_row = q + static_cast<long long>(qr.x + t) * p.q_row_stride + head * p.q_head_stride;
-      val = *reinterpret_cast<const uint4*>(q_row + 8 * c);
-      if (p.rotary_cos != nullptr && c < p.rotary_half / 4)
-        val = rotate_chunk<T>(val, q_row, c, rotary_pos(p, b, p.causal ? t : 0), p);
+    for (int idx = tid; idx < kRows * kChunks; idx += 128) {
+      const int r = idx / kChunks, c = idx % kChunks;
+      uint4 val = make_uint4(0u, 0u, 0u, 0u);
+      if (r < rows_here) {
+        const int pr = row0 + r;
+        const int t = pr / group, head = kv_head * group + pr % group;
+        val = *reinterpret_cast<const uint4*>(q8 + static_cast<long long>(qr.x + t) * p.q_row_stride +
+                                              head * p.q_head_stride + 16 * c);
+      }
+      const int phys = kD == 128 ? c ^ (r & 7) : c ^ ((r >> 1) & 3);
+      *reinterpret_cast<uint4*>(smem_q + r * kD + (phys << 4)) = val;
     }
-    *reinterpret_cast<uint4*>(smem_q + (c >> 3) * kQHalfBytes + r * 128 + (((c & 7) ^ (r & 7)) << 4)) = val;
+  } else {
+    constexpr int kChunks = kD / 8;  // 16-byte chunks per row
+#pragma unroll 4
+    for (int idx = tid; idx < kRows * kChunks; idx += 128) {
+      const int r = idx / kChunks, c = idx % kChunks;
+      uint4 val = make_uint4(0u, 0u, 0u, 0u);
+      if (r < rows_here) {
+        const int pr = row0 + r;
+        const int t = pr / group, head = kv_head * group + pr % group;
+        const T* q_row = q + static_cast<long long>(qr.x + t) * p.q_row_stride + head * p.q_head_stride;
+        val = *reinterpret_cast<const uint4*>(q_row + 8 * c);
+        if (p.rotary_cos != nullptr && c < p.rotary_half / 4)
+          val = rotate_chunk<T>(val, q_row, c, rotary_pos(p, b, p.causal ? t : 0), p);
+      }
+      *reinterpret_cast<uint4*>(smem_q + (c >> 3) * kQHalfBytes + r * 128 + (((c & 7) ^ (r & 7)) << 4)) = val;
+    }
   }
   fence_proxy_async_smem();
   named_bar_sync(1, 128);
@@ -438,40 +514,76 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   float m2[2] = {-CUDART_INF_F, -CUDART_INF_F};
   float l[2] = {0.f, 0.f};
   float t2 = p.scale_log2;
-  if constexpr (kFp8) t2 *= p.k_descale[b * p.hkv + kv_head];
+  if constexpr (kQ8) t2 = t2 * p.q_descale[b * p.hkv + kv_head] * p.k_descale[b * p.hkv + kv_head];
+  else if constexpr (kFp8) t2 *= p.k_descale[b * p.hkv + kv_head];
 
-  const uint64_t q_desc = gmma_desc(smem_u32(smem_q), 0);         // K-major A
-  const uint64_t k_desc0 = gmma_desc(smem_u32(smem_kv), 0);       // K tile, K-major B
+  // K-major A; e4m3 queries: the e4m3 Q tile, and the fp8 K slots (K-major B) instead of the T ones
+  const uint64_t q_desc = kQ8 ? f8_desc<kD>(smem_q) : gmma_desc(smem_u32(smem_q), 0);
+  const uint64_t k_desc0 = kQ8 ? f8_desc<kD>(smem_f8) : gmma_desc(smem_u32(smem_kv), 0);  // K tile, K-major B
   const uint64_t v_desc0 = gmma_desc(smem_u32(smem_kv), kKHalfBytes);  // V tile, MN-major B
 
   uint32_t slot = 0, phase = 0;
+  [[maybe_unused]] uint32_t kf_slot = 0, kf_phase = 0;  // e4m3 queries: K of tile jj is fp8 item 2 jj
   for (int jj = 0; jj < n_tiles; ++jj) {
-    const uint32_t k_slot = slot, k_phase = phase;
-    if (++slot == kSlots) {
-      slot = 0;
-      phase ^= 1;
-    }
-    const uint32_t v_slot = slot, v_phase = phase;
-    if (++slot == kSlots) {
-      slot = 0;
-      phase ^= 1;
+    uint32_t k_slot, k_phase, v_slot, v_phase;
+    if constexpr (kQ8) {
+      k_slot = kf_slot;
+      k_phase = kf_phase;
+      kf_slot += 2;
+      if (kf_slot >= L::kSlots) {
+        kf_slot -= L::kSlots;
+        kf_phase ^= 1;
+      }
+      v_slot = slot;
+      v_phase = phase;
+      if (++slot == kSlots) {
+        slot = 0;
+        phase ^= 1;
+      }
+    } else {
+      k_slot = slot;
+      k_phase = phase;
+      if (++slot == kSlots) {
+        slot = 0;
+        phase ^= 1;
+      }
+      v_slot = slot;
+      v_phase = phase;
+      if (++slot == kSlots) {
+        slot = 0;
+        phase ^= 1;
+      }
     }
     const int key0 = (j0 + jj) * kTile;
 
     // ---- S = Q K^T
-    mbar_wait(&bars->kv_full[k_slot], k_phase);
     float s[64];
-    const uint64_t k_desc = gmma_desc_add(k_desc0, k_slot * kSlotBytes);
-    wgmma_fence();
+    if constexpr (kQ8) {
+      mbar_wait(&bars->f8_full[k_slot], k_phase);
+      const uint64_t k_desc = gmma_desc_add(k_desc0, k_slot * L::kSlotBytes);
+      wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < kD / 16; ++k)
-      Gmma<T>::template ss128<0, 0>(s, gmma_desc_add(q_desc, (k >> 2) * kQHalfBytes + (k & 3) * 32),
-                                    gmma_desc_add(k_desc, (k >> 2) * kKHalfBytes + (k & 3) * 32), k > 0);
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(s);
-    __syncwarp();
-    if (warp_leader) mbar_arrive(&bars->kv_empty[k_slot]);
+      for (int k = 0; k < kD / 32; ++k)
+        wgmma_ss_m64n128k32_e4m3(s, gmma_desc_add(q_desc, 32 * k), gmma_desc_add(k_desc, 32 * k), k > 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s);
+      __syncwarp();
+      if (warp_leader) mbar_arrive(&bars->f8_empty[k_slot]);  // the fp8 K slot goes straight back to TMA
+    } else {
+      mbar_wait(&bars->kv_full[k_slot], k_phase);
+      const uint64_t k_desc = gmma_desc_add(k_desc0, k_slot * kSlotBytes);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kD / 16; ++k)
+        Gmma<T>::template ss128<0, 0>(s, gmma_desc_add(q_desc, (k >> 2) * kQHalfBytes + (k & 3) * 32),
+                                      gmma_desc_add(k_desc, (k >> 2) * kKHalfBytes + (k & 3) * 32), k > 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s);
+      __syncwarp();
+      if (warp_leader) mbar_arrive(&bars->kv_empty[k_slot]);
+    }
 
     // ---- mask keys at or past each row's limit
 #pragma unroll
@@ -701,14 +813,24 @@ __global__ void decode_combine_kernel(const float* parts, long long part_stride,
 }  // namespace dec
 
 const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_cache, const TensorView& v_cache,
-                              const void* k_new, const void* v_new, const DecodeParams& p, int n_splits, int head_dim,
-                              cudaStream_t stream) {
+                              const void* k_new, const void* v_new, int new_dtype, const DecodeParams& p,
+                              int n_splits, int head_dim, cudaStream_t stream) {
   if (head_dim != 64 && head_dim != 128) return "the sm_90a decode kernel is instantiated for head_dim 64 and 128";
-  if (dtype != kDtypeBF16 && dtype != kDtypeFP16) return "the sm_90a decode kernel takes bf16 / fp16";
+  if (dtype != kDtypeBF16 && dtype != kDtypeFP16 && dtype != kDtypeE4M3)
+    return "the sm_90a decode kernel takes a bf16 / fp16 / e4m3 q";
   const bool fp8 = cache_dtype == kDtypeE4M3;
+  const bool q8 = dtype == kDtypeE4M3;
   if (!fp8 && cache_dtype != dtype) return "the caches must have q's dtype or be e4m3";
   if (fp8 != (p.k_descale != nullptr && p.v_descale != nullptr))
     return "e4m3 caches need k / v descales, and only e4m3 caches take them";
+  if (q8 != (p.q_descale != nullptr)) return "e4m3 queries need q_descale, and only they take it";
+  if (q8 && p.rotary_cos != nullptr) return "rotary needs a bf16 / fp16 q: rotate before quantising";
+  if (k_new != nullptr) {
+    const bool new_ok = new_dtype == dtype || (fp8 && new_dtype == kDtypeE4M3) ||
+                        (q8 && (new_dtype == kDtypeBF16 || new_dtype == kDtypeFP16));
+    if (!new_ok) return "k_new / v_new must have q's dtype, be e4m3 over an e4m3 cache, or bf16 / fp16 with an e4m3 q";
+    if (new_dtype == kDtypeE4M3 && p.rotary_cos != nullptr) return "rotary needs a bf16 / fp16 k_new";
+  }
   if (p.hkv <= 0 || p.hq % p.hkv != 0) return "query heads must be a multiple of kv heads";
   if (k_cache.row_stride != v_cache.row_stride || k_cache.head_stride != v_cache.head_stride)
     return "k_cache and v_cache must have the same strides";
@@ -744,7 +866,10 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
     else if (!fp8)
       dec::decode_append_kernel<__half><<<agrid, 128, 0, stream>>>(kc, vc, k_cache.row_stride * 2,
                                                                    k_cache.head_stride * 2, kn, vn, p, head_dim * 2);
-    else if (dtype == kDtypeBF16)
+    else if (new_dtype == kDtypeE4M3)  // pre-quantised k / v: their bytes, as they are (never rotated)
+      dec::decode_append_kernel<__nv_bfloat16><<<agrid, 128, 0, stream>>>(kc, vc, k_cache.row_stride,
+                                                                          k_cache.head_stride, kn, vn, p, head_dim);
+    else if (new_dtype == kDtypeBF16)
       dec::decode_append_e4m3_kernel<<<agrid, 128, 0, stream>>>(
           kc, vc, k_cache.row_stride, k_cache.head_stride, static_cast<const __nv_bfloat16*>(k_new),
           static_cast<const __nv_bfloat16*>(v_new), p, head_dim);
@@ -770,10 +895,18 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
     using T = decltype(t);
     constexpr bool kFp8 = decltype(f8)::value;
     const int threads = kFp8 ? dec::kThreadsFp8 : dec::kThreads;
-    if (head_dim == 128) launch(dec::decode_kernel<T, 128, kFp8>, dec::smem_bytes<128, kFp8>(), threads);
-    else launch(dec::decode_kernel<T, 64, kFp8>, dec::smem_bytes<64, kFp8>(), threads);
+    if (head_dim == 128)
+      launch(dec::decode_kernel<T, 128, kFp8, false>, dec::smem_bytes<128, kFp8, false>(), threads);
+    else launch(dec::decode_kernel<T, 64, kFp8, false>, dec::smem_bytes<64, kFp8, false>(), threads);
   };
-  if (dtype == kDtypeBF16) {
+  if (q8) {  // e4m3 queries over an e4m3 cache: bf16 P V
+    if (head_dim == 128)
+      launch(dec::decode_kernel<__nv_bfloat16, 128, true, true>, dec::smem_bytes<128, true, true>(),
+             dec::kThreadsFp8);
+    else
+      launch(dec::decode_kernel<__nv_bfloat16, 64, true, true>, dec::smem_bytes<64, true, true>(),
+             dec::kThreadsFp8);
+  } else if (dtype == kDtypeBF16) {
     if (fp8) pick(__nv_bfloat16{}, std::true_type{});
     else pick(__nv_bfloat16{}, std::false_type{});
   } else {

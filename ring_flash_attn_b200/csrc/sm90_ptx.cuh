@@ -131,6 +131,12 @@ __device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes
   return static_cast<uint64_t>((saddr & 0x3FFFF) >> 4) | (static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16) |
          (static_cast<uint64_t>(1024 >> 4) << 32) | (static_cast<uint64_t>(1) << 62);
 }
+// The same for a K-major operand of 64-byte rows under TMA's 64-byte swizzle (layout type 2): 8-row groups of 512
+// bytes, so SBO = 512; LBO is unused, since a K step (32 e4m3 elements) stays inside the row.
+__device__ __forceinline__ uint64_t gmma_desc_sw64(uint32_t saddr) {
+  return static_cast<uint64_t>((saddr & 0x3FFFF) >> 4) | (static_cast<uint64_t>(512 >> 4) << 32) |
+         (static_cast<uint64_t>(2) << 62);
+}
 // Start-address field of a descriptor moved by `bytes` (multiples of 16; never crosses the 18-bit field).
 __device__ __forceinline__ uint64_t gmma_desc_add(uint64_t desc, uint32_t bytes) { return desc + (bytes >> 4); }
 

@@ -76,14 +76,14 @@ _warned = set()
 def _kernel_takes(q: Tensor) -> bool:
     if not cuda_ext.available_for(q):
         return False
-    if q.dtype in (torch.bfloat16, torch.float16) and q.shape[-1] in KERNEL_HEAD_DIMS:
+    if q.dtype in (torch.bfloat16, torch.float16, torch.float8_e4m3fn) and q.shape[-1] in KERNEL_HEAD_DIMS:
         return True
     key = (q.dtype, q.shape[-1])
     if key not in _warned:
         _warned.add(key)
         warnings.warn(f"cp_flash_attn_with_kvcache: no sm_90a decode kernel for {q.dtype} with head_dim {q.shape[-1]} "
-                      f"(instantiated: bf16 / fp16, head_dim {KERNEL_HEAD_DIMS}); running the dense torch path",
-                      RuntimeWarning, stacklevel=3)
+                      f"(instantiated: bf16 / fp16, and e4m3 over e4m3 caches, head_dim {KERNEL_HEAD_DIMS}); running "
+                      "the dense torch path", RuntimeWarning, stacklevel=3)
     return False
 
 
@@ -103,20 +103,28 @@ def _capacity(k_cache: Tensor, block_table: Optional[Tensor]) -> int:
     return k_cache.shape[1] if block_table is None else block_table.shape[1] * k_cache.shape[1]
 
 
+def _out_dtype(q: Tensor) -> torch.dtype:
+    """``out``'s dtype: q's, or bf16 for an e4m3 ``q`` (flash-attn 3's rule)."""
+    return torch.bfloat16 if q.dtype == torch.float8_e4m3fn else q.dtype
+
+
 def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor, k: Optional[Tensor],
                   v: Optional[Tensor], causal: bool, softmax_scale: float, pg=None, world: int = 1,
                   splits: Optional[int] = None, block_table: Optional[Tensor] = None,
                   k_descale: Optional[Tensor] = None, v_descale: Optional[Tensor] = None,
                   cu_seqlens_q: Optional[Tensor] = None, max_seqlen_q: Optional[int] = None,
                   rotary_cos: Optional[Tensor] = None, rotary_sin: Optional[Tensor] = None,
-                  rotary_seqlens: Optional[Tensor] = None, rotary_interleaved: bool = True) -> Tuple[Tensor, Tensor]:
+                  rotary_seqlens: Optional[Tensor] = None, rotary_interleaved: bool = True,
+                  q_descale: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
     """Local split-KV kernel (appending ``k`` / ``v`` first when given), then the combine over the splits and, for
     ``world > 1``, over the gathered per-rank partials.  ``splits`` overrides :func:`num_splits`.  With
     ``block_table`` the caches are page pools (see :func:`cp_flash_attn_with_kvcache`).  e4m3 caches take contiguous
     fp32 ``(B, Hkv)`` ``k_descale`` / ``v_descale``.  With ``cu_seqlens_q`` (and ``max_seqlen_q``) ``q`` / ``k`` /
     ``v`` are varlen ``(total_q, H, D)`` and the result is ``out (total_q, Hq, D)``, ``lse (Hq, total_q)``.  With
     ``rotary_cos`` / ``rotary_sin`` (and ``rotary_seqlens``, required here) the kernel rotates ``q`` as it loads it
-    and ``k`` before it stores it, as :func:`apply_rotary` does, at positions clamped to the tables."""
+    and ``k`` before it stores it, as :func:`apply_rotary` does, at positions clamped to the tables.  An e4m3 ``q``
+    (over e4m3 caches) takes a contiguous fp32 ``(B, Hkv)`` ``q_descale`` and gives a bf16 ``out``; e4m3 ``k`` / ``v``
+    over e4m3 caches are stored as they are."""
     C = cuda_ext.load()
     varlen = cu_seqlens_q is not None
     if varlen:  # the partials are the uniform layout at batch 1, Sq = total_q
@@ -141,16 +149,17 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
     # every split's partial starts 8-byte aligned (the kernel stores out as float2): rows * Hq * (D + 1) is odd when
     # rows and Hq are
     parts = torch.empty((splits, size + size % 2), dtype=torch.float32, device=q.device)[:, :size]
+    extra = () if q_descale is None else (q_descale,)  # decode_fwd takes q_descale only for an e4m3 q
     C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts, block_table, k_descale,
                  v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0, rotary_cos, rotary_sin, rotary_seqlens,
-                 bool(rotary_interleaved))
+                 bool(rotary_interleaved), *extra)
     cuda_ext.note_launch(2 if k is not None else 1)
     if world > 1:
         mine = torch.empty(size, dtype=torch.float32, device=q.device)
         C.decode_combine(parts, mine[:n_out].view(rows_b, rows_sq, hq, d), mine[n_out:].view(rows_b, hq, rows_sq))
         cuda_ext.note_launch()
         parts = _gather(mine, pg, world)
-    out = torch.empty(q.shape, dtype=q.dtype, device=q.device)
+    out = torch.empty(q.shape, dtype=_out_dtype(q), device=q.device)
     lse = torch.empty((rows_b, hq, rows_sq), dtype=torch.float32, device=q.device)
     C.decode_combine(parts, out.view(rows_b, rows_sq, hq, d), lse)
     cuda_ext.note_launch()
@@ -215,8 +224,9 @@ def _varlen_spans(cu_seqlens_q: Tensor, total_q: int, max_seqlen_q: int):
 
 
 def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table=None,
-                  k_descale=None, v_descale=None, cu_seqlens_q=None, max_seqlen_q=0, rotary=None):
+                  k_descale=None, v_descale=None, cu_seqlens_q=None, max_seqlen_q=0, rotary=None, q_descale=None):
     # every sequence is a (first row, count) span of the packed rows: (b * Sq, Sq) for a uniform q
+    out_dtype = _out_dtype(q)
     b = cache_seqlens.shape[0]
     hq, d = q.shape[-2:]
     if cu_seqlens_q is not None:
@@ -233,6 +243,10 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
         q = apply_rotary(q, cos, sin, q_pos, interleaved)
         if k is not None:
             k = apply_rotary(k, cos, sin, key_pos, interleaved)
+    if q_descale is not None:  # e4m3 q: the query it stands for, q.float() * q_descale[b, h // G]
+        g = hq // q_descale.shape[1]
+        q = torch.cat([q[lo:lo + n].float() * q_descale[i].repeat_interleave(g)[:, None]
+                       for i, (lo, n) in enumerate(spans)])
     rows = q.shape[0]
     s_cap = _capacity(k_cache, block_table)
     lens = [max(0, min(int(x), s_cap)) for x in cache_seqlens.tolist()]
@@ -240,7 +254,7 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
     table = block_table.tolist() if block_table is not None else None
     fp8 = k_descale is not None
     if k is not None:  # rows past the capacity (or whose page is outside the pool) are dropped, as in the kernel path
-        if fp8:
+        if fp8 and k.dtype != torch.float8_e4m3fn:  # pre-quantised e4m3 k / v are stored as they are
             k = torch.cat([quantize_e4m3(k[lo:lo + n], k_descale[i]) for i, (lo, n) in enumerate(spans)])
             v = torch.cat([quantize_e4m3(v[lo:lo + n], v_descale[i]) for i, (lo, n) in enumerate(spans)])
         for i, n in enumerate(lens):
@@ -286,7 +300,7 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
     if cu_seqlens_q is None:  # back to (B, Sq, Hq, D) and (B, Hq, Sq)
         out = out.reshape(b, sq, hq, d)
         lse = lse.reshape(hq, b, sq).permute(1, 0, 2).contiguous()
-    return out.to(q.dtype), lse
+    return out.to(out_dtype), lse
 
 
 # ----------------------------------------------------------------------------------------------
@@ -299,14 +313,14 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
               block_table: Optional[Tensor], k_descale: Optional[Tensor], v_descale: Optional[Tensor],
               cu_seqlens_q: Optional[Tensor], max_seqlen_q: int, rotary_cos: Optional[Tensor] = None,
               rotary_sin: Optional[Tensor] = None, rotary_seqlens: Optional[Tensor] = None,
-              rotary_interleaved: bool = True) -> Tuple[Tensor, Tensor]:
-    """q (B, Sq, Hq, D) -> (out (B, Sq, Hq, D) in q.dtype, lse (B, Hq, Sq) fp32).  ``k`` / ``v`` are appended to
-    the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's name ("" = world);
-    with ``block_table`` the caches are this rank's page pools; e4m3 caches come with contiguous fp32 (B, Hkv)
-    ``k_descale`` / ``v_descale``.  With ``cu_seqlens_q`` q / k / v are varlen (total_q, H, D), out is
+              rotary_interleaved: bool = True, q_descale: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+    """q (B, Sq, Hq, D) -> (out (B, Sq, Hq, D) in q.dtype (bf16 for an e4m3 q), lse (B, Hq, Sq) fp32).  ``k`` /
+    ``v`` are appended to the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's
+    name ("" = world); with ``block_table`` the caches are this rank's page pools; e4m3 caches come with contiguous
+    fp32 (B, Hkv) ``k_descale`` / ``v_descale``.  With ``cu_seqlens_q`` q / k / v are varlen (total_q, H, D), out is
     (total_q, Hq, D) and lse (Hq, total_q); ``max_seqlen_q`` bounds the counts (0 when uniform).  With
     ``rotary_cos`` / ``rotary_sin`` / ``rotary_seqlens``, every rank rotates q and the append rank rotates k before
-    it stores it."""
+    it stores it.  An e4m3 q comes with a contiguous fp32 (B, Hkv) ``q_descale``."""
     pg = resolve_group(group)
     rank, world = group_info(pg)
     if k is not None and not 0 <= append_rank < world:
@@ -318,21 +332,22 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
                              block_table=block_table, k_descale=k_descale, v_descale=v_descale,
                              cu_seqlens_q=cu_seqlens_q, max_seqlen_q=max_seqlen_q, rotary_cos=rotary_cos,
                              rotary_sin=rotary_sin, rotary_seqlens=rotary_seqlens,
-                             rotary_interleaved=rotary_interleaved)
+                             rotary_interleaved=rotary_interleaved, q_descale=q_descale)
     rotary = None if rotary_cos is None else (rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved)
     return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table,
-                         k_descale, v_descale, cu_seqlens_q, max_seqlen_q, rotary)
+                         k_descale, v_descale, cu_seqlens_q, max_seqlen_q, rotary, q_descale)
 
 
 @cp_decode.register_fake
 def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group, block_table, k_descale,
       v_descale, cu_seqlens_q, max_seqlen_q, rotary_cos=None, rotary_sin=None, rotary_seqlens=None,
-      rotary_interleaved=True):
+      rotary_interleaved=True, q_descale=None):
+    out = q.new_empty(q.shape, dtype=_out_dtype(q))
     if cu_seqlens_q is not None:
         total_q, hq, _ = q.shape
-        return q.new_empty(q.shape), q.new_empty((hq, total_q), dtype=torch.float32)
+        return out, q.new_empty((hq, total_q), dtype=torch.float32)
     b, sq, hq, _ = q.shape
-    return q.new_empty(q.shape), q.new_empty((b, hq, sq), dtype=torch.float32)
+    return out, q.new_empty((b, hq, sq), dtype=torch.float32)
 
 
 def _valid_page_size(ps: int) -> bool:
@@ -405,7 +420,7 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
                                softmax_scale=None, causal=True, return_softmax_lse=False, group=None, *,
                                block_table=None, k_descale=None, v_descale=None, cu_seqlens_q=None,
                                max_seqlen_q=None, rotary_cos=None, rotary_sin=None, rotary_interleaved=True,
-                               rotary_seqlens=None, window_size=(-1, -1), alibi_slopes=None):
+                               rotary_seqlens=None, window_size=(-1, -1), alibi_slopes=None, q_descale=None):
     """Decode attention of new query tokens against a KV cache sharded over ``group`` (modelled on flash-attn's
     ``flash_attn_with_kvcache``).  Inference only: no gradient.
 
@@ -429,8 +444,17 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
       graph replay uses their current contents) and are not validated: non-finite or non-positive descales give an
       undefined result.  The appended ``k`` / ``v`` stay in q's dtype and are stored as
       ``(x.float() / descale).clamp(-448, 448).to(torch.float8_e4m3fn)``.  An e4m3 cache holds twice the tokens of
-      a bf16 one and a decode step reads half the bytes.  Descales given with a bf16 / fp16 cache, fp8 queries,
-      ``float8_e5m2`` caches, mixed cache dtypes and fp8 caches with an fp32 ``q`` raise ``ValueError``.
+      a bf16 one and a decode step reads half the bytes.  Descales given with a bf16 / fp16 cache, ``float8_e5m2``
+      caches, mixed cache dtypes and fp8 caches with an fp32 ``q`` raise ``ValueError``.
+    * fp8 queries (flash-attn 3's ``q_descale``): over e4m3 caches, ``q`` may be ``torch.float8_e4m3fn``, with
+      ``q_descale`` required: an fp32 tensor on q's device of shape ``()``, ``(Hkv,)`` or ``(B, Hkv)``, the same on
+      every rank.  The query stands for ``q.float() * q_descale[b, h // G]``, and ``out`` is bf16.  The kernel runs
+      ``Q K^T`` as an e4m3 tensor-core product straight on the cache's fp8 K tiles and widens only V.  ``q_descale``
+      is read on the device only (a CUDA graph replay uses its current contents) and is not validated.  With an e4m3
+      ``q``, ``k`` / ``v`` may be ``torch.float8_e4m3fn`` (both): their bytes are stored as they are, and they stand
+      for ``k.float() * k_descale`` like the cache; bf16 / fp16 ``k`` / ``v`` are quantised as above.  ``q_descale``
+      with a bf16 / fp16 ``q``, an e4m3 ``q`` without it or over a bf16 / fp16 cache, a ``float8_e5m2`` ``q`` and
+      rotary with an e4m3 ``q`` (rotate before quantising) raise ``ValueError``.
     * ``cache_seqlens`` ``(B,)`` int32 on q's device: valid rows of this rank's shard (0 = empty shard).
     * ``k`` / ``v`` ``(B, Sq, Hkv, D)``, optional, the same on every rank: written in place into the caches of rank
       ``append_rank`` only, at rows ``[cache_seqlens[b], cache_seqlens[b] + Sq)``, before attention (rows past
@@ -452,11 +476,12 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
       access outside ``q``, ``k``, ``v`` or the caches.  The dense path raises ``ValueError`` for them
       (``cu_seqlens_q[0] != 0``, a decreasing entry, ``cu_seqlens_q[B] != total_q``, a count above
       ``max_seqlen_q``).  Long chunks are correct but not efficient: every 64-row tile reads the whole shard.
-    * Returns ``out`` ``(B, Sq, Hq, D)`` in q.dtype, and ``softmax_lse`` ``(B, Hq, Sq)`` fp32 when
-      ``return_softmax_lse``.  Both are bitwise identical on every rank.
+    * Returns ``out`` ``(B, Sq, Hq, D)`` in q.dtype (bf16 for an e4m3 ``q``), and ``softmax_lse`` ``(B, Hq, Sq)``
+      fp32 when ``return_softmax_lse``.  Both are bitwise identical on every rank.
     * ``window_size``, ``alibi_slopes``, ``D > 128`` and ``Hq % Hkv != 0`` raise ``ValueError``.  The sm_90a kernel
-      covers a bf16 / fp16 ``q`` with ``D`` in {64, 128}, over caches in q's dtype or e4m3; other head sizes run the
-      dense torch path with a one-time warning.
+      covers a bf16 / fp16 ``q`` with ``D`` in {64, 128}, over caches in q's dtype or e4m3, and an e4m3 ``q`` over
+      e4m3 caches; other head sizes run the dense torch path with a one-time warning (an e4m3 ``q`` dequantised with
+      ``q_descale``).
     * Rotary embeddings (flash-attn's ``rotary_cos`` / ``rotary_sin`` / ``rotary_interleaved``, and flash-attn 3's
       ``rotary_seqlens``): ``rotary_cos`` / ``rotary_sin`` are contiguous ``(seqlen_ro, rotary_dim / 2)`` tensors in
       q's dtype on q's device, the same on every rank; ``rotary_dim`` is a multiple of 16 and at most ``D``, and
@@ -508,16 +533,27 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
         raise ValueError(f"cu_seqlens_q must be a contiguous (B + 1,) = ({b + 1},) int32 tensor")
     if varlen and cu_seqlens_q.device != q.device:
         raise ValueError("cu_seqlens_q must be on q's device")
-    if q.element_size() == 1:
-        raise ValueError("cp_flash_attn_with_kvcache: fp8 queries are not supported")
+    q8 = q.dtype == torch.float8_e4m3fn
+    if q.element_size() == 1 and not q8:
+        raise ValueError(f"cp_flash_attn_with_kvcache: fp8 queries must be torch.float8_e4m3fn, not {q.dtype}")
+    if q8 and not (k_cache.dtype == v_cache.dtype == torch.float8_e4m3fn):
+        raise ValueError("cp_flash_attn_with_kvcache: fp8 (e4m3) queries need e4m3 caches, not "
+                         f"{k_cache.dtype} / {v_cache.dtype}")
+    if q8:
+        if q_descale is None:
+            raise ValueError("cp_flash_attn_with_kvcache: fp8 queries (e4m3) need q_descale (fp32, shape (), (Hkv,) "
+                             "or (B, Hkv))")
+        q_descale = _check_descale("q_descale", q_descale, q, b, hkv)
+    elif q_descale is not None:
+        raise ValueError("q_descale is only taken with an fp8 (float8_e4m3fn) q")
     if k_cache.element_size() == 1 or v_cache.element_size() == 1:
         if k_cache.dtype != v_cache.dtype:
             raise ValueError(f"fp8 caches: k_cache ({k_cache.dtype}) and v_cache ({v_cache.dtype}) must both be "
                              "torch.float8_e4m3fn")
         if k_cache.dtype != torch.float8_e4m3fn:
             raise ValueError(f"fp8 caches must be torch.float8_e4m3fn, not {k_cache.dtype}")
-        if q.dtype not in (torch.bfloat16, torch.float16):
-            raise ValueError(f"fp8 caches need a bf16 / fp16 q, not {q.dtype}")
+        if q.dtype not in (torch.bfloat16, torch.float16, torch.float8_e4m3fn):
+            raise ValueError(f"fp8 caches need a bf16 / fp16 q, or an e4m3 q with q_descale, not {q.dtype}")
         k_descale = _check_descale("k_descale", k_descale, q, b, hkv)
         v_descale = _check_descale("v_descale", v_descale, q, b, hkv)
     else:
@@ -539,15 +575,23 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
     if k is not None:
         if append_rank is None:
             raise ValueError("append_rank is required when k / v are given")
+        if q8:  # pre-quantised e4m3 k / v (stored as they are), or bf16 / fp16 ones (quantised as they are stored)
+            if k.dtype != v.dtype or k.dtype not in (torch.float8_e4m3fn, torch.bfloat16, torch.float16):
+                raise ValueError(f"with an e4m3 q, k / v must both be float8_e4m3fn, bf16 or fp16, not {k.dtype} / "
+                                 f"{v.dtype}")
         for t in (k, v):
-            if varlen and (tuple(t.shape) != (total_q, hkv, d) or t.dtype != q.dtype):
+            dtype_ok = t.dtype == k.dtype if q8 else t.dtype == q.dtype
+            if varlen and (tuple(t.shape) != (total_q, hkv, d) or not dtype_ok):
                 raise ValueError(f"with cu_seqlens_q, k / v must be (total_q, Hkv, D) = {(total_q, hkv, d)} in "
                                  "q's dtype")
-            if not varlen and (tuple(t.shape) != (b, sq, hkv, d) or t.dtype != q.dtype):
+            if not varlen and (tuple(t.shape) != (b, sq, hkv, d) or not dtype_ok):
                 raise ValueError(f"k / v must be (B, Sq, Hkv, D) = {(b, sq, hkv, d)} in q's dtype")
     elif append_rank is not None:
         raise ValueError("append_rank must be None when no k / v are given")
     if rotary_cos is not None or rotary_sin is not None:
+        if q8:
+            raise ValueError("rotary_cos / rotary_sin need a bf16 / fp16 q: the rotation belongs before quantisation, "
+                             "so rotate q and k, then quantise them")
         rotary_seqlens = _check_rotary(rotary_cos, rotary_sin, rotary_seqlens, q, b, d, cache_seqlens, group)
         if k is None:
             raise ValueError("rotary_cos / rotary_sin need k / v: the rotation applies to the new tokens")
@@ -557,5 +601,5 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
     out, lse = cp_decode(q, k_cache, v_cache, cache_seqlens, k, v, -1 if append_rank is None else int(append_rank),
                          scale, bool(causal), group_name(group), block_table, k_descale, v_descale, cu_seqlens_q,
                          max_seqlen_q if varlen else 0, rotary_cos, rotary_sin, rotary_seqlens,
-                         bool(rotary_interleaved))
+                         bool(rotary_interleaved), q_descale)
     return (out, lse) if return_softmax_lse else out
