@@ -23,6 +23,13 @@ With ``--rotary`` every configuration also times, in the same loop, a RoPE decod
 (the shard then holds the cache length): the fused call (``rotary_cos`` / ``rotary_sin``, non-interleaved, rotary_dim
 = head_dim), the same step done without it (``apply_rotary`` on q and k with torch ops, then a plain call), and the
 plain call alone; and reports whether the fused and unfused outputs are bitwise equal.
+With ``--cache-slots N`` every configuration also times, in the same loop, an appending step over a pool of N cache
+slots (each of the cache length) where the B sequences use a seeded random subset of slots (``cache_batch_idx``),
+the same step on a B-slot cache with the same contents, and what a caller without ``cache_batch_idx`` must do:
+``index_select`` the B slots out of the pool, the plain call, and ``index_copy_`` them back; and reports whether
+the slot and plain outputs are bitwise equal.  With ``--leftpad P`` it also times a call whose sequences have P
+pad rows below their keys (``cache_leftpad``) against the plain call on the same number of valid rows.  Both arms run
+over the cache and query dtypes that ``--kv-dtype`` / ``--q-dtype`` select.
 
     python benchmark/bench_decode.py                      # B in {1, 8}, caches of 32K..512K tokens per rank
     python benchmark/bench_decode.py --page-size 16       # also the paged kernel, pages of 16 rows
@@ -30,6 +37,8 @@ plain call alone; and reports whether the fused and unfused outputs are bitwise 
     python benchmark/bench_decode.py --kv-dtype e4m3 --q-dtype e4m3   # and the fp8-query kernel
     python benchmark/bench_decode.py --mixed-chunk 64     # also a ragged batch: one 64-token chunk + decodes
     python benchmark/bench_decode.py --rotary             # also the fused RoPE step against the unfused one
+    python benchmark/bench_decode.py --cache 32768 --cache-slots 16   # also a slot pool against gather / scatter
+    python benchmark/bench_decode.py --leftpad 1000       # also a left-padded call against the plain one
     torchrun --nproc-per-node 2 benchmark/bench_decode.py
     python benchmark/bench_decode.py --dry-run            # shapes and byte counts only (no GPU)
 """
@@ -69,8 +78,18 @@ def parse_args(argv=None):
                          "call padded to Sq = C and the uniform Sq = 1 call")
     ap.add_argument("--rotary", action="store_true",
                     help="also time a RoPE step: the fused call, the torch rotation + a plain call, the plain call")
+    ap.add_argument("--cache-slots", type=int, default=None, metavar="N",
+                    help="also time a step over an N-slot cache pool (cache_batch_idx) against the plain call and "
+                         "the index_select / call / index_copy_ workaround")
+    ap.add_argument("--leftpad", type=int, default=None, metavar="P",
+                    help="also time a call with P pad rows per sequence (cache_leftpad) against the plain call on "
+                         "the same number of valid rows")
     ap.add_argument("--dry-run", action="store_true")
     args = ap.parse_args(argv)
+    if args.cache_slots is not None and args.cache_slots < max(args.batch):
+        ap.error("--cache-slots must be at least the largest --batch (the sequences use distinct slots)")
+    if args.leftpad is not None and not 0 <= args.leftpad < min(args.cache):
+        ap.error("--leftpad must be in [0, the smallest --cache)")
     if args.q_dtype == "e4m3" and args.kv_dtype != "e4m3":
         ap.error("--q-dtype e4m3 needs --kv-dtype e4m3 (fp8 queries run over e4m3 caches only)")
     return args
@@ -105,6 +124,12 @@ def shapes(args, sm_count):
                            varlen_kv_bytes=(chunk_tiles + b - 1) * shard, padded_kv_bytes=b * chunk_tiles * shard)
             if args.rotary:  # positions cache_tokens - Sq + t of a table with one row per cached token
                 cfg.update(rotary_dim=args.head_dim, rotary_interleaved=False, seqlen_ro=s)
+            slot_bytes = cfg["fp8_kv_bytes"] if args.kv_dtype == "e4m3" else cfg["kv_bytes"]  # B slots of K + V
+            if args.cache_slots:  # the workaround reads and writes the B slots twice (gather, then scatter)
+                cfg.update(cache_slots=args.cache_slots, pool_bytes=slot_bytes // b * args.cache_slots,
+                           gather_scatter_bytes=4 * slot_bytes)
+            if args.leftpad is not None:
+                cfg.update(leftpad=args.leftpad, leftpad_kv_bytes=slot_bytes // s * (s - args.leftpad))
             yield cfg
 
 
@@ -262,6 +287,54 @@ def main():
             def rot_plain():
                 return dec.kernel_decode(q, kc, vc, sl_app, k_new, v_new, True, scale)
 
+        if args.cache_slots or args.leftpad is not None:  # over the cache and query dtypes the flags select
+            if q8:
+                bq, bk, bv, bkw = q_e4m3, k8, v8, dict(k_descale=kd, v_descale=vd, q_descale=qd)
+            elif fp8:
+                bq, bk, bv, bkw = q, k8, v8, dict(k_descale=kd, v_descale=vd)
+            else:
+                bq, bk, bv, bkw = q, kc, vc, {}
+
+        if args.cache_slots:  # B distinct slots of an N-slot pool hold the B-slot cache's rows
+            n_slots = args.cache_slots
+            idx = torch.randperm(n_slots, generator=torch.Generator().manual_seed(rank))[:b].to(dev)
+            idx32 = idx.to(torch.int32)
+            raw_k, raw_v = bk.view(torch.uint8), bv.view(torch.uint8)
+            pool_k = torch.zeros((n_slots,) + tuple(raw_k.shape[1:]), dtype=torch.uint8, device=dev)
+            pool_v = torch.zeros_like(pool_k)
+            pool_k[idx], pool_v[idx] = raw_k, raw_v
+            pool_k, pool_v = pool_k.view(bk.dtype), pool_v.view(bk.dtype)
+            # append Sq new tokens at rows [s - Sq, s) every call (bf16 k / v: quantised into an e4m3 cache)
+            kn_app = torch.randn(b, args.sq, args.hkv, d, device=dev, dtype=torch.bfloat16)
+            vn_app = torch.randn_like(kn_app)
+            sl_app = torch.full((b,), s - args.sq, dtype=torch.int32, device=dev)
+
+            def slot_call():
+                return dec.kernel_decode(bq, pool_k, pool_v, sl_app, kn_app, vn_app, True, scale,
+                                         cache_batch_idx=idx32, **bkw)
+
+            def slot_plain():
+                return dec.kernel_decode(bq, bk, bv, sl_app, kn_app, vn_app, True, scale, **bkw)
+
+            def slot_gather():  # without cache_batch_idx: gather the B slots, a plain call, scatter them back
+                gk = pool_k.view(torch.uint8).index_select(0, idx)
+                gv = pool_v.view(torch.uint8).index_select(0, idx)
+                r = dec.kernel_decode(bq, gk.view(bk.dtype), gv.view(bk.dtype), sl_app, kn_app, vn_app, True, scale,
+                                      **bkw)
+                pool_k.view(torch.uint8).index_copy_(0, idx, gk)
+                pool_v.view(torch.uint8).index_copy_(0, idx, gv)
+                return r
+
+        if args.leftpad is not None:  # P pad rows below every sequence's keys, against s - P rows from row 0
+            lpad = torch.full((b,), args.leftpad, dtype=torch.int32, device=dev)
+            sl_short = torch.full((b,), s - args.leftpad, dtype=torch.int32, device=dev)
+
+            def lp_call():
+                return dec.kernel_decode(bq, bk, bv, sl, None, None, True, scale, cache_leftpad=lpad, **bkw)
+
+            def lp_plain():
+                return dec.kernel_decode(bq, bk, bv, sl_short, None, None, True, scale, **bkw)
+
         # SDPA reads the same shard through (B, H, S, D) views
         qt, kt, vt = q.transpose(1, 2), kc.transpose(1, 2), vc.transpose(1, 2)
 
@@ -281,6 +354,8 @@ def main():
                 rows["paged_q8"] = []
         mixed_rows = {"mixed_varlen": [], "mixed_padded": [], "mixed_decode_only": []}
         rot_rows = {"rotary_fused": [], "rotary_unfused": [], "rotary_plain": []}
+        slot_rows = {"slots": [], "slots_plain": [], "slots_gather_scatter": []}
+        lp_rows = {"leftpad": [], "leftpad_plain": []}
         sdpa_err = None
         for _ in range(3):  # alternate them in one run
             rows["ours"].append(time_us(ours, args.iters, args.warmup))
@@ -292,6 +367,13 @@ def main():
                 rot_rows["rotary_fused"].append(time_us(rot_fused, args.iters, args.warmup))
                 rot_rows["rotary_unfused"].append(time_us(rot_unfused, args.iters, args.warmup))
                 rot_rows["rotary_plain"].append(time_us(rot_plain, args.iters, args.warmup))
+            if args.cache_slots:
+                slot_rows["slots"].append(time_us(slot_call, args.iters, args.warmup))
+                slot_rows["slots_plain"].append(time_us(slot_plain, args.iters, args.warmup))
+                slot_rows["slots_gather_scatter"].append(time_us(slot_gather, args.iters, args.warmup))
+            if args.leftpad is not None:
+                lp_rows["leftpad"].append(time_us(lp_call, args.iters, args.warmup))
+                lp_rows["leftpad_plain"].append(time_us(lp_plain, args.iters, args.warmup))
             if args.page_size:
                 rows["paged"].append(time_us(paged, args.iters, args.warmup))
             if fp8:
@@ -335,6 +417,21 @@ def main():
             res["rotary_fused_over_plain"] = round(res["rotary_fused_us"] / res["rotary_plain_us"], 3)
             res["rotary_speedup_vs_unfused"] = round(res["rotary_unfused_us"] / res["rotary_fused_us"], 3)
             res["rotary_fused_equal_unfused"] = all(torch.equal(x, y) for x, y in zip(rot_fused(), rot_unfused()))
+        if args.cache_slots or args.leftpad is not None:
+            res["slot_arms_q_dtype"], res["slot_arms_kv_dtype"] = args.q_dtype, args.kv_dtype
+        if args.cache_slots:
+            for k, ts in slot_rows.items():
+                res[f"{k}_us"] = round(min(ts), 2)
+                res[f"{k}_us_all"] = [round(t, 2) for t in ts]
+            res["slots_over_plain"] = round(res["slots_us"] / res["slots_plain_us"], 3)
+            res["slots_speedup_vs_gather_scatter"] = round(res["slots_gather_scatter_us"] / res["slots_us"], 3)
+            # every arm appended the same rows to the same contents, so the caches still agree
+            res["slots_equal_plain"] = all(torch.equal(x, y) for x, y in zip(slot_call(), slot_plain()))
+        if args.leftpad is not None:
+            for k, ts in lp_rows.items():
+                res[f"{k}_us"] = round(min(ts), 2)
+                res[f"{k}_us_all"] = [round(t, 2) for t in ts]
+            res["leftpad_over_plain"] = round(res["leftpad_us"] / res["leftpad_plain_us"], 3)
         if args.page_size:
             res["paged_equal_contiguous"] = all(torch.equal(x, y) for x, y in zip(paged(), ours()))
         if fp8:
@@ -373,6 +470,10 @@ def main():
             del k_new, v_new, cos, sin
         if args.page_size:
             del pk, pv
+        if args.cache_slots:
+            del pool_k, pool_v, kn_app, vn_app
+        if args.cache_slots or args.leftpad is not None:
+            del bq, bk, bv, bkw
         if fp8:
             del k8, v8
             if q8:

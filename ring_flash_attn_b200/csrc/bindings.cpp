@@ -409,6 +409,9 @@ at::Tensor lse_unflatten(const at::Tensor& lse, const at::Tensor& cu, int64_t ma
 // q and the appended k are rotated (see DecodeParams); rotary_seqlens is read on the device only.  q may be
 // float8_e4m3fn over e4m3 caches, with q_descale fp32 (B, Hkv) contiguous on q's device (partials of a bf16 P V);
 // k_new / v_new may be float8_e4m3fn over e4m3 caches (stored as they are), or bf16 / fp16 with an e4m3 q.
+// cache_batch_idx (B,) int32 (contiguous caches only): sequence b reads and appends slot cache_batch_idx[b] of
+// (B_cache, S_cap, Hkv, D) caches; cache_leftpad (B,) int32: its keys start at that row.  Both are read on the device
+// only (see DecodeParams).
 void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
                 const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
                 double scale, at::Tensor& part, const c10::optional<at::Tensor>& block_table,
@@ -416,7 +419,8 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
                 const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q,
                 const c10::optional<at::Tensor>& rotary_cos, const c10::optional<at::Tensor>& rotary_sin,
                 const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved,
-                const c10::optional<at::Tensor>& q_descale) {
+                const c10::optional<at::Tensor>& q_descale, const c10::optional<at::Tensor>& cache_batch_idx,
+                const c10::optional<at::Tensor>& cache_leftpad) {
   const c10::cuda::CUDAGuard guard(q_in.device());
   const bool varlen = cu_seqlens_q.has_value();
   TORCH_CHECK(q_in.dim() == (varlen ? 3 : 4), "decode_fwd: q must be (B, Sq, Hq, D), or (total_q, Hq, D) with "
@@ -449,7 +453,18 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
   const int64_t s_cap = paged ? block_table->size(1) * page_size : k_cache.size(1);
   const int64_t hkv = k_cache.size(2);
   const int64_t cache_rows = k_cache.size(0) * k_cache.size(1);
-  TORCH_CHECK((paged || k_cache.size(0) == B) && k_cache.size(3) == d, "decode_fwd: cache shape does not match q");
+  const bool slots = cache_batch_idx.has_value();
+  TORCH_CHECK((paged || slots || k_cache.size(0) == B) && k_cache.size(3) == d,
+              "decode_fwd: cache shape does not match q");
+  TORCH_CHECK(!paged || (!slots && !cache_leftpad.has_value()),
+              "decode_fwd: cache_batch_idx and cache_leftpad take a contiguous cache, not a block table");
+  for (const c10::optional<at::Tensor>* t : {&cache_batch_idx, &cache_leftpad})
+    TORCH_CHECK(!t->has_value() || ((*t)->scalar_type() == at::kInt && (*t)->device() == q.device() &&
+                                    (*t)->dim() == 1 && (*t)->numel() == B && (*t)->is_contiguous()),
+                "decode_fwd: cache_batch_idx / cache_leftpad must be (B,) int32 contiguous on q's device");
+  // the TMA row coordinate of a contiguous cache is an int32
+  TORCH_CHECK(paged || !slots || cache_rows < (int64_t(1) << 31),
+              "decode_fwd: with cache_batch_idx, B_cache * S_cap must be below 2^31");
   TORCH_CHECK(q.stride(3) == 1 && (varlen || q.stride(0) == sq * q.stride(1)),
               "decode_fwd: q must be (B, Sq) mergeable");
   TORCH_CHECK((q.stride(1) * q.element_size()) % 16 == 0 && (q.stride(2) * q.element_size()) % 16 == 0 &&
@@ -564,6 +579,11 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
     p.seqlen_ro = static_cast<int>(rc.size(0));
     p.rotary_interleaved = rotary_interleaved ? 1 : 0;
   }
+  if (slots) {
+    p.cache_batch_idx = cache_batch_idx->data_ptr<int>();
+    p.cache_batch = static_cast<int>(k_cache.size(0));
+  }
+  if (cache_leftpad.has_value()) p.cache_leftpad = cache_leftpad->data_ptr<int>();
   const TensorView kv{k_cache.data_ptr(), cache_rows, static_cast<int>(hkv), k_cache.stride(1), k_cache.stride(2)};
   const TensorView vv{v_cache.data_ptr(), cache_rows, static_cast<int>(hkv), v_cache.stride(1), v_cache.stride(2)};
   check(rfa::decode_fwd_launch(q8 ? rfa::kDtypeE4M3 : dtype_code(q), fp8 ? rfa::kDtypeE4M3 : dtype_code(q), kv, vv,
@@ -636,6 +656,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("lse_flatten", &lse_flatten);
   m.def("lse_unflatten", &lse_unflatten);
   m.def("decode_fwd", &decode_fwd);
+  // the same without cache_batch_idx / cache_leftpad
+  m.def("decode_fwd", [](const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
+                         const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
+                         double scale, at::Tensor& part, const c10::optional<at::Tensor>& block_table,
+                         const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale,
+                         const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q,
+                         const c10::optional<at::Tensor>& rotary_cos, const c10::optional<at::Tensor>& rotary_sin,
+                         const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved,
+                         const c10::optional<at::Tensor>& q_descale) {
+    decode_fwd(q, k_cache, v_cache, seqlens, k_new, v_new, causal, scale, part, block_table, k_descale, v_descale,
+               cu_seqlens_q, max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, q_descale,
+               c10::nullopt, c10::nullopt);
+  });
   // the same without q_descale (a bf16 / fp16 q)
   m.def("decode_fwd", [](const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
                          const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
@@ -645,7 +678,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                          const c10::optional<at::Tensor>& rotary_cos, const c10::optional<at::Tensor>& rotary_sin,
                          const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved) {
     decode_fwd(q, k_cache, v_cache, seqlens, k_new, v_new, causal, scale, part, block_table, k_descale, v_descale,
-               cu_seqlens_q, max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, c10::nullopt);
+               cu_seqlens_q, max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, c10::nullopt,
+               c10::nullopt, c10::nullopt);
   });
   m.def("decode_combine", &decode_combine);
   rfa::bind_peer_mem(m);

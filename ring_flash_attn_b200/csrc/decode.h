@@ -50,6 +50,13 @@ struct DecodeParams {
   int rotary_interleaved;
   // e4m3 queries (only over e4m3 caches): q holds x / q_descale[b, kv head]; nullptr for a bf16 / fp16 q
   const float* q_descale;  // (B, Hkv) contiguous; read on the device only
+  // Contiguous caches only, both read on the device only.  Sequence b reads and appends slot cache_batch_idx[b] of a
+  // (cache_batch, s_cap, Hkv, D) cache (nullptr: slot b); a slot outside [0, cache_batch) sees no key and drops its
+  // append.  Its keys are rows [cache_leftpad[b], seqlens[b]) of the slot plus the appended rows (nullptr: from row
+  // 0); the pad is clamped to [0, seqlens[b]].  Everything else (seqlens, descales, rotary) stays indexed by b.
+  const int* cache_batch_idx;  // (B,)
+  int cache_batch;
+  const int* cache_leftpad;  // (B,)
 };
 
 // Appends k_new / v_new (B, Sq, Hkv, D), contiguous, in q's dtype, at rows [seqlens[b], seqlens[b] + Sq) of the

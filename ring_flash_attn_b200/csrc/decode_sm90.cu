@@ -40,6 +40,13 @@
 // the sequence's token count otherwise).  Cache rows at or past that limit are never read into a result: their K
 // columns are masked to -inf and their V rows are zeroed in shared memory before P V (the cache may hold anything
 // there, NaN included).
+//
+// Cache slots and left padding (contiguous caches): sequence b's keys live in slot cache_batch_idx[b] and start at
+// row lp = cache_leftpad[b].  Each CTA resolves both once and then runs on keys relative to lp: seqlens[b] - lp valid
+// rows under a capacity of S_cap - lp, so the key loop, masks and split ranges are those of a plain call on the
+// slot shifted down by lp rows.  Only the producer's row coordinate (slot * S_cap + lp + key) and the append's target
+// row see the slot and the pad.  Tile rows past the last visible key may reach into the next slot or past the tensor
+// (TMA fills those with zeros); they are discarded like any row at or past the limit.
 #include <math_constants.h>
 
 #include <type_traits>
@@ -93,11 +100,12 @@ struct LoadRing {
   static constexpr int kSlotBytes = kTile * kSubTiles * kRowBytes;
 };
 
-// Keys of the shard visible to token t of a sequence with n_q new tokens (see the file comment), at most the capacity.
-__device__ __forceinline__ int key_limit(const DecodeParams& p, int seqlen, int n_q, int t) {
+// Keys of the shard visible to token t of a sequence with n_q new tokens (see the file comment), at most cap, all
+// counted from the sequence's first key row.
+__device__ __forceinline__ int key_limit(const DecodeParams& p, int seqlen, int cap, int n_q, int t) {
   const int n_vis = p.n_new == 0 ? 0 : (p.causal ? t + 1 : n_q);
   const int lim = seqlen + n_vis;
-  return lim < p.s_cap ? lim : p.s_cap;
+  return lim < cap ? lim : cap;
 }
 
 __device__ __forceinline__ int clamp_to(int x, int lo, int hi) { return x < lo ? lo : (x > hi ? hi : x); }
@@ -340,8 +348,17 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   const int rows_here = n_rows - row0 < kRows ? n_rows - row0 : kRows;
   int seqlen = p.seqlens[b];
   seqlen = seqlen < 0 ? 0 : (seqlen > p.s_cap ? p.s_cap : seqlen);
+  // the sequence's cache slot and first key row; keys below are counted from lp (see the file comment)
+  int cache_slot = b, cap = p.s_cap;
+  if (p.cache_batch_idx != nullptr) {
+    cache_slot = __ldg(p.cache_batch_idx + b);
+    if (cache_slot < 0 || cache_slot >= p.cache_batch) seqlen = cap = 0;  // no slot: no key, nor any appended one
+  }
+  const int lp = p.cache_leftpad != nullptr ? clamp_to(__ldg(p.cache_leftpad + b), 0, seqlen) : 0;
+  seqlen -= lp;
+  cap -= lp;
   // the last row of the tile sees the most keys (the limit never decreases with t)
-  const int kmax = key_limit(p, seqlen, qr.y, (row0 + rows_here - 1) / group);
+  const int kmax = key_limit(p, seqlen, cap, qr.y, (row0 + rows_here - 1) / group);
   const int j0 = split * p.tiles_per_split;
   int j1 = (kmax + kTile - 1) / kTile;
   if (j1 > j0 + p.tiles_per_split) j1 = j0 + p.tiles_per_split;
@@ -384,7 +401,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
     } else if (threadIdx.x == kProducer) {
       uint32_t slot = 0, phase = 0;
       for (int jj = 0; jj < n_tiles; ++jj) {
-        const int row = b * p.s_cap + (j0 + jj) * kTile;  // rows past the tensor's end arrive as zeros
+        const int row = cache_slot * p.s_cap + lp + (j0 + jj) * kTile;  // rows past the tensor's end arrive as zeros
         for (int kv = 0; kv < 2; ++kv) {
           mbar_wait(&load_empty[slot], phase ^ 1);
           uint8_t* dst = smem_load + slot * L::kSlotBytes;
@@ -506,7 +523,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int r = r_base + 8 * h;
-    lim[h] = r < rows_here ? key_limit(p, seqlen, qr.y, (row0 + r) / group) : 0;
+    lim[h] = r < rows_here ? key_limit(p, seqlen, cap, qr.y, (row0 + r) / group) : 0;
   }
   float o[kD / 2];
 #pragma unroll
@@ -690,12 +707,16 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   }
 }
 
-// Cache row of new key t of sequence b (the pool row with a block table), or -1 when the row is dropped: past the
-// capacity, or with a page id outside the pool.
+// Cache row of new key t of sequence b (the pool row with a block table, a row of slot cache_batch_idx[b] with one),
+// or -1 when the row is dropped: past the capacity, with a page id outside the pool, or with a slot outside the cache.
 __device__ __forceinline__ long long append_row(const DecodeParams& p, int b, int t) {
   const int row = p.seqlens[b] + t;
   if (row < 0 || row >= p.s_cap) return -1;
-  if (p.page_size == 0) return static_cast<long long>(b) * p.s_cap + row;
+  if (p.page_size == 0) {
+    const int slot = p.cache_batch_idx != nullptr ? __ldg(p.cache_batch_idx + b) : b;
+    if (slot < 0 || (p.cache_batch_idx != nullptr && slot >= p.cache_batch)) return -1;
+    return static_cast<long long>(slot) * p.s_cap + row;
+  }
   const int page = p.block_table[b * p.bt_stride + row / p.page_size];
   if (page < 0 || page >= p.num_pages) return -1;
   return static_cast<long long>(page) * p.page_size + row % p.page_size;

@@ -115,7 +115,8 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
                   cu_seqlens_q: Optional[Tensor] = None, max_seqlen_q: Optional[int] = None,
                   rotary_cos: Optional[Tensor] = None, rotary_sin: Optional[Tensor] = None,
                   rotary_seqlens: Optional[Tensor] = None, rotary_interleaved: bool = True,
-                  q_descale: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+                  q_descale: Optional[Tensor] = None, cache_batch_idx: Optional[Tensor] = None,
+                  cache_leftpad: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
     """Local split-KV kernel (appending ``k`` / ``v`` first when given), then the combine over the splits and, for
     ``world > 1``, over the gathered per-rank partials.  ``splits`` overrides :func:`num_splits`.  With
     ``block_table`` the caches are page pools (see :func:`cp_flash_attn_with_kvcache`).  e4m3 caches take contiguous
@@ -124,7 +125,8 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
     ``rotary_cos`` / ``rotary_sin`` (and ``rotary_seqlens``, required here) the kernel rotates ``q`` as it loads it
     and ``k`` before it stores it, as :func:`apply_rotary` does, at positions clamped to the tables.  An e4m3 ``q``
     (over e4m3 caches) takes a contiguous fp32 ``(B, Hkv)`` ``q_descale`` and gives a bf16 ``out``; e4m3 ``k`` / ``v``
-    over e4m3 caches are stored as they are."""
+    over e4m3 caches are stored as they are.  ``cache_batch_idx`` / ``cache_leftpad`` (contiguous ``(B,)`` int32,
+    contiguous caches only) select each sequence's cache slot and first key row, read on the device only."""
     C = cuda_ext.load()
     varlen = cu_seqlens_q is not None
     if varlen:  # the partials are the uniform layout at batch 1, Sq = total_q
@@ -150,6 +152,8 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
     # rows and Hq are
     parts = torch.empty((splits, size + size % 2), dtype=torch.float32, device=q.device)[:, :size]
     extra = () if q_descale is None else (q_descale,)  # decode_fwd takes q_descale only for an e4m3 q
+    if cache_batch_idx is not None or cache_leftpad is not None:
+        extra = (q_descale, cache_batch_idx, cache_leftpad)
     C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts, block_table, k_descale,
                  v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0, rotary_cos, rotary_sin, rotary_seqlens,
                  bool(rotary_interleaved), *extra)
@@ -224,7 +228,8 @@ def _varlen_spans(cu_seqlens_q: Tensor, total_q: int, max_seqlen_q: int):
 
 
 def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table=None,
-                  k_descale=None, v_descale=None, cu_seqlens_q=None, max_seqlen_q=0, rotary=None, q_descale=None):
+                  k_descale=None, v_descale=None, cu_seqlens_q=None, max_seqlen_q=0, rotary=None, q_descale=None,
+                  cache_batch_idx=None, cache_leftpad=None):
     # every sequence is a (first row, count) span of the packed rows: (b * Sq, Sq) for a uniform q
     out_dtype = _out_dtype(q)
     b = cache_seqlens.shape[0]
@@ -253,6 +258,14 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
     ps, n_pages = k_cache.shape[1], k_cache.shape[0]
     table = block_table.tolist() if block_table is not None else None
     fp8 = k_descale is not None
+    # sequence i's cache slot and first key row (the kernel path reads both on the device only and does not check them)
+    slots = list(range(b)) if cache_batch_idx is None else cache_batch_idx.tolist()
+    pads = [0] * b if cache_leftpad is None else cache_leftpad.tolist()
+    for i, (slot, lp) in enumerate(zip(slots, pads)):
+        if cache_batch_idx is not None and not 0 <= slot < n_pages:
+            raise ValueError(f"cache_batch_idx[{i}] = {slot} is outside the {n_pages}-slot cache")
+        if not 0 <= lp <= lens[i]:
+            raise ValueError(f"cache_leftpad[{i}] = {lp} is outside [0, cache_seqlens[{i}]] = [0, {lens[i]}]")
     if k is not None:  # rows past the capacity (or whose page is outside the pool) are dropped, as in the kernel path
         if fp8 and k.dtype != torch.float8_e4m3fn:  # pre-quantised e4m3 k / v are stored as they are
             k = torch.cat([quantize_e4m3(k[lo:lo + n], k_descale[i]) for i, (lo, n) in enumerate(spans)])
@@ -261,8 +274,8 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
             lo, cnt = spans[i]
             m = min(cnt, s_cap - n)
             if table is None:
-                k_cache[i, n:n + m] = k[lo:lo + m]
-                v_cache[i, n:n + m] = v[lo:lo + m]
+                k_cache[slots[i], n:n + m] = k[lo:lo + m]
+                v_cache[slots[i], n:n + m] = v[lo:lo + m]
                 continue
             for t in range(m):
                 page = table[i][(n + t) // ps]
@@ -275,10 +288,11 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
         lo, cnt = spans[i]
         n_new = cnt if k is not None else 0
         n_keys = min(n + n_new, s_cap)
-        if n_keys == 0 or cnt == 0:
+        lp = pads[i]  # rows [lp, n_keys) of the slot
+        if n_keys == lp or cnt == 0:
             continue
         if table is None:
-            kk, vv = k_cache[i, :n_keys], v_cache[i, :n_keys]
+            kk, vv = k_cache[slots[i], lp:n_keys], v_cache[slots[i], lp:n_keys]
         else:  # the pages holding the visible rows, in table order
             pages = table[i][:-(-n_keys // ps)]
             if not all(0 <= x < n_pages for x in pages):
@@ -286,8 +300,8 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
             kk, vv = k_cache[pages].flatten(0, 1)[:n_keys], v_cache[pages].flatten(0, 1)[:n_keys]
         if fp8:  # the dequantised rows
             kk, vv = kk.float() * k_descale[i][:, None], vv.float() * v_descale[i][:, None]
-        # appended key u (row n + u) is visible to token t iff u <= t, i.e. row j <= t + n
-        diag = n if (n_new and causal) else None
+        # appended key u (row n + u) is visible to token t iff u <= t, i.e. row j <= t + n (j counted from lp)
+        diag = n - lp if (n_new and causal) else None
         out[lo:lo + cnt], lse[:, lo:lo + cnt] = block_fwd(q[lo:lo + cnt], kk, vv, softmax_scale, diag)
     if world > 1:
         parts = _gather(torch.cat([out.reshape(-1), lse.reshape(-1)]), pg, world)
@@ -313,14 +327,16 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
               block_table: Optional[Tensor], k_descale: Optional[Tensor], v_descale: Optional[Tensor],
               cu_seqlens_q: Optional[Tensor], max_seqlen_q: int, rotary_cos: Optional[Tensor] = None,
               rotary_sin: Optional[Tensor] = None, rotary_seqlens: Optional[Tensor] = None,
-              rotary_interleaved: bool = True, q_descale: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+              rotary_interleaved: bool = True, q_descale: Optional[Tensor] = None,
+              cache_batch_idx: Optional[Tensor] = None, cache_leftpad: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
     """q (B, Sq, Hq, D) -> (out (B, Sq, Hq, D) in q.dtype (bf16 for an e4m3 q), lse (B, Hq, Sq) fp32).  ``k`` /
     ``v`` are appended to the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's
     name ("" = world); with ``block_table`` the caches are this rank's page pools; e4m3 caches come with contiguous
     fp32 (B, Hkv) ``k_descale`` / ``v_descale``.  With ``cu_seqlens_q`` q / k / v are varlen (total_q, H, D), out is
     (total_q, Hq, D) and lse (Hq, total_q); ``max_seqlen_q`` bounds the counts (0 when uniform).  With
     ``rotary_cos`` / ``rotary_sin`` / ``rotary_seqlens``, every rank rotates q and the append rank rotates k before
-    it stores it.  An e4m3 q comes with a contiguous fp32 (B, Hkv) ``q_descale``."""
+    it stores it.  An e4m3 q comes with a contiguous fp32 (B, Hkv) ``q_descale``.  ``cache_batch_idx`` /
+    ``cache_leftpad`` (B,) int32 pick each sequence's cache slot and first key row."""
     pg = resolve_group(group)
     rank, world = group_info(pg)
     if k is not None and not 0 <= append_rank < world:
@@ -332,16 +348,18 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
                              block_table=block_table, k_descale=k_descale, v_descale=v_descale,
                              cu_seqlens_q=cu_seqlens_q, max_seqlen_q=max_seqlen_q, rotary_cos=rotary_cos,
                              rotary_sin=rotary_sin, rotary_seqlens=rotary_seqlens,
-                             rotary_interleaved=rotary_interleaved, q_descale=q_descale)
+                             rotary_interleaved=rotary_interleaved, q_descale=q_descale,
+                             cache_batch_idx=cache_batch_idx, cache_leftpad=cache_leftpad)
     rotary = None if rotary_cos is None else (rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved)
     return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table,
-                         k_descale, v_descale, cu_seqlens_q, max_seqlen_q, rotary, q_descale)
+                         k_descale, v_descale, cu_seqlens_q, max_seqlen_q, rotary, q_descale, cache_batch_idx,
+                         cache_leftpad)
 
 
 @cp_decode.register_fake
 def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group, block_table, k_descale,
       v_descale, cu_seqlens_q, max_seqlen_q, rotary_cos=None, rotary_sin=None, rotary_seqlens=None,
-      rotary_interleaved=True, q_descale=None):
+      rotary_interleaved=True, q_descale=None, cache_batch_idx=None, cache_leftpad=None):
     out = q.new_empty(q.shape, dtype=_out_dtype(q))
     if cu_seqlens_q is not None:
         total_q, hq, _ = q.shape
@@ -383,6 +401,13 @@ def _check_descale(name, x, q, b, hkv):
     return x.expand(b, hkv).contiguous()
 
 
+def _check_cache_index(name, x, q, b):
+    if (not isinstance(x, Tensor) or x.dtype != torch.int32 or tuple(x.shape) != (b,) or not x.is_contiguous()):
+        raise ValueError(f"{name} must be a contiguous (B,) = ({b},) int32 tensor")
+    if x.device != q.device:
+        raise ValueError(f"{name} must be on q's device")
+
+
 def _check_rotary(cos, sin, rotary_seqlens, q, b, d, cache_seqlens, group):
     """Checks the rotary tables and returns the (B,) positions the kernels read: ``rotary_seqlens``, or
     ``cache_seqlens`` in a one-rank group."""
@@ -420,7 +445,8 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
                                softmax_scale=None, causal=True, return_softmax_lse=False, group=None, *,
                                block_table=None, k_descale=None, v_descale=None, cu_seqlens_q=None,
                                max_seqlen_q=None, rotary_cos=None, rotary_sin=None, rotary_interleaved=True,
-                               rotary_seqlens=None, window_size=(-1, -1), alibi_slopes=None, q_descale=None):
+                               rotary_seqlens=None, window_size=(-1, -1), alibi_slopes=None, q_descale=None,
+                               cache_batch_idx=None, cache_leftpad=None):
     """Decode attention of new query tokens against a KV cache sharded over ``group`` (modelled on flash-attn's
     ``flash_attn_with_kvcache``).  Inference only: no gradient.
 
@@ -456,6 +482,23 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
       with a bf16 / fp16 ``q``, an e4m3 ``q`` without it or over a bf16 / fp16 cache, a ``float8_e5m2`` ``q`` and
       rotary with an e4m3 ``q`` (rotate before quantising) raise ``ValueError``.
     * ``cache_seqlens`` ``(B,)`` int32 on q's device: valid rows of this rank's shard (0 = empty shard).
+    * ``cache_batch_idx`` ``(B,)`` int32 on q's device, contiguous, optional (flash-attn's argument): sequence ``b``
+      reads and appends slot ``cache_batch_idx[b]`` of ``(B_cache, S_cap, Hkv, D)`` caches, for any
+      ``B_cache >= 1`` with ``B_cache * S_cap < 2**31`` (a pool of slots decoded a changing subset at a time, or
+      several sequences reading one shared prompt).  ``cache_seqlens``, ``cache_leftpad``, the descales and
+      ``rotary_seqlens`` stay indexed by ``b``, not by the slot.  Slots not named are never read or written.
+      Duplicate indices are allowed; with ``k`` / ``v``, which duplicate's rows land in the shared slot is
+      unspecified.  Each rank passes its own.  Not with ``block_table`` (the table already gives every sequence
+      its own pages).
+    * ``cache_leftpad`` ``(B,)`` int32 on q's device, contiguous, optional (flash-attn's argument): the keys of
+      sequence ``b`` are rows ``[cache_leftpad[b], cache_seqlens[b])`` of its slot plus the appended rows, which
+      still start at ``cache_seqlens[b]``; rows below the pad may hold anything, NaN included, and are never loaded.
+      A left-padded batch prefilled with the ring, zigzag or stripe layout keeps its pad tokens in a leading row
+      range of every shard, so each rank passes the count of its own pad rows.  Rotary positions do not change.
+      Not with ``block_table``.  The kernel path reads both tensors on the device only (a CUDA graph replay uses
+      their current contents) and does not validate them: an index outside ``[0, B_cache)`` or a pad outside
+      ``[0, cache_seqlens[b]]`` gives an undefined result but no access outside the caches (the sequence sees no key
+      on this rank and its append is dropped; the pad is clamped).  The dense path raises ``ValueError`` for both.
     * ``k`` / ``v`` ``(B, Sq, Hkv, D)``, optional, the same on every rank: written in place into the caches of rank
       ``append_rank`` only, at rows ``[cache_seqlens[b], cache_seqlens[b] + Sq)``, before attention (rows past
       ``S_cap`` are dropped).  The caller advances ``cache_seqlens``.  ``append_rank`` is required with ``k`` / ``v``
@@ -526,7 +569,20 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
     else:
         b, sq, hq, d = q.shape
     hkv = k_cache.shape[2]
-    if (block_table is None and k_cache.shape[0] != b) or k_cache.shape[3] != d or sq < 1:
+    if block_table is not None and cache_batch_idx is not None:
+        raise ValueError("cache_batch_idx takes a contiguous cache: a paged cache does not support cache_batch_idx "
+                         "(the block table already gives every sequence its own pages)")
+    if block_table is not None and cache_leftpad is not None:
+        raise ValueError("cache_leftpad takes a contiguous cache: a paged cache does not support cache_leftpad")
+    if cache_batch_idx is not None:
+        _check_cache_index("cache_batch_idx", cache_batch_idx, q, b)
+        if k_cache.shape[0] < 1 or k_cache.shape[0] * k_cache.shape[1] >= 2 ** 31:
+            raise ValueError(f"with cache_batch_idx, B_cache * S_cap = {k_cache.shape[0]} * {k_cache.shape[1]} must "
+                             "be between 1 and 2^31 - 1")
+    if cache_leftpad is not None:
+        _check_cache_index("cache_leftpad", cache_leftpad, q, b)
+    if ((block_table is None and cache_batch_idx is None and k_cache.shape[0] != b) or k_cache.shape[3] != d
+            or sq < 1):
         raise ValueError(f"q {tuple(q.shape)} does not match the cache {tuple(k_cache.shape)}")
     if varlen and (not isinstance(cu_seqlens_q, Tensor) or cu_seqlens_q.dtype != torch.int32
                    or tuple(cu_seqlens_q.shape) != (b + 1,) or not cu_seqlens_q.is_contiguous()):
@@ -601,5 +657,5 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
     out, lse = cp_decode(q, k_cache, v_cache, cache_seqlens, k, v, -1 if append_rank is None else int(append_rank),
                          scale, bool(causal), group_name(group), block_table, k_descale, v_descale, cu_seqlens_q,
                          max_seqlen_q if varlen else 0, rotary_cos, rotary_sin, rotary_seqlens,
-                         bool(rotary_interleaved), q_descale)
+                         bool(rotary_interleaved), q_descale, cache_batch_idx, cache_leftpad)
     return (out, lse) if return_softmax_lse else out
