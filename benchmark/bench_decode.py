@@ -30,6 +30,13 @@ the same step on a B-slot cache with the same contents, and what a caller withou
 the slot and plain outputs are bitwise equal.  With ``--leftpad P`` it also times a call whose sequences have P
 pad rows below their keys (``cache_leftpad``) against the plain call on the same number of valid rows.  Both arms run
 over the cache and query dtypes that ``--kv-dtype`` / ``--q-dtype`` select.
+With ``--shared-prefix L --samples n`` the run times shared-prefix decoding instead: P prompts (``--prompts``) of L
+tokens per rank, n samples each, every sample with its own ``--suffix`` rows and one appended token per call, in three
+arms with the same contents, alternating in one loop: the prefix call (``prefix_k_cache`` / ``prefix_v_cache``), the
+prompt copied into each sample's contiguous cache ahead of its suffix (a plain call), and paged caches of 128-row pages
+whose block tables share the prompt's pages.  Each line reports the HBM bytes each arm must read (from shapes), the
+largest difference between the arms' outputs, and the card's name, power limit and maximum SM clock (read in one
+``nvidia-smi`` query).  ``--kv-dtype e4m3`` runs the three arms over e4m3 caches with one descale per kv head.
 
     python benchmark/bench_decode.py                      # B in {1, 8}, caches of 32K..512K tokens per rank
     python benchmark/bench_decode.py --page-size 16       # also the paged kernel, pages of 16 rows
@@ -40,6 +47,7 @@ over the cache and query dtypes that ``--kv-dtype`` / ``--q-dtype`` select.
     python benchmark/bench_decode.py --cache 32768 --cache-slots 16   # also a slot pool against gather / scatter
     python benchmark/bench_decode.py --leftpad 1000       # also a left-padded call against the plain one
     torchrun --nproc-per-node 2 benchmark/bench_decode.py
+    python benchmark/bench_decode.py --shared-prefix 32768 131072 --samples 4 16   # one prompt, n samples
     python benchmark/bench_decode.py --dry-run            # shapes and byte counts only (no GPU)
 """
 import argparse
@@ -84,8 +92,16 @@ def parse_args(argv=None):
     ap.add_argument("--leftpad", type=int, default=None, metavar="P",
                     help="also time a call with P pad rows per sequence (cache_leftpad) against the plain call on "
                          "the same number of valid rows")
+    ap.add_argument("--shared-prefix", type=int, nargs="+", default=None, metavar="L",
+                    help="time shared-prefix decoding instead: prompts of L tokens per rank (see --samples)")
+    ap.add_argument("--samples", type=int, nargs="+", default=[4, 16], help="samples per prompt (--shared-prefix)")
+    ap.add_argument("--prompts", type=int, nargs="+", default=[1], help="prompts P per call (--shared-prefix)")
+    ap.add_argument("--suffix", type=int, default=256, help="each sample's own cached rows (--shared-prefix)")
     ap.add_argument("--dry-run", action="store_true")
     args = ap.parse_args(argv)
+    if args.shared_prefix is not None and (min(args.shared_prefix) < 1 or args.suffix < 1 or min(args.samples) < 1
+                                           or min(args.prompts) < 1):
+        ap.error("--shared-prefix, --samples, --prompts and --suffix must be positive")
     if args.cache_slots is not None and args.cache_slots < max(args.batch):
         ap.error("--cache-slots must be at least the largest --batch (the sequences use distinct slots)")
     if args.leftpad is not None and not 0 <= args.leftpad < min(args.cache):
@@ -133,6 +149,132 @@ def shapes(args, sm_count):
             yield cfg
 
 
+PREFIX_PAGE = 128  # rows per page of the paged arm
+
+
+def prefix_shapes(args, sm_count):
+    """One dict per shared-prefix configuration: shapes, split counts and the K + V bytes each arm must read."""
+    hkv, d, g = args.hkv, args.head_dim, args.hq // args.hkv
+    eb = 1 if args.kv_dtype == "e4m3" else 2
+    row = hkv * d * 2 * eb  # K + V bytes of one cached token
+    for n_prompts in args.prompts:
+        for length in args.shared_prefix:
+            for n in args.samples:
+                b, suf = n_prompts * n, args.suffix
+                slots = dec.prefix_tile_slots(n, 1, args.hq, hkv)
+                yield dict(shared_prefix=length, samples=n, prompts=n_prompts, batch=b, suffix=suf, sq=1, hq=args.hq,
+                           hkv=hkv, head_dim=d, kv_dtype=args.kv_dtype, page_size=PREFIX_PAGE,
+                           suffix_splits=dec.num_splits(b, 1, args.hq, hkv, suf, sm_count),
+                           prefix_splits=dec.num_splits_prefix(n_prompts, slots, hkv, length, sm_count),
+                           plain_splits=dec.num_splits(b, 1, args.hq, hkv, length + suf, sm_count),
+                           rows_per_prefix_tile=min(n * g, dec.ROWS_PER_CTA),
+                           prefix_bytes=(n_prompts * length + b * suf) * row,
+                           copied_bytes=b * (length + suf) * row, paged_bytes=b * (length + suf) * row)
+
+
+def card_settings():
+    """(name, power limit, max SM clock) of this process's GPU, read in one nvidia-smi query."""
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader",
+                            "-i", str(torch.cuda.current_device())], stdout=subprocess.PIPE, text=True, timeout=30)
+        name, power, clock = (x.strip() for x in r.stdout.strip().split(","))
+    except (OSError, subprocess.SubprocessError, ValueError):
+        name, power, clock = torch.cuda.get_device_name(0), "unknown", "unknown"
+    return name, power, clock
+
+
+def shared_prefix_main(args):
+    """The three shared-prefix arms, alternating in one loop (see the module docstring)."""
+    if args.dry_run:
+        for cfg in prefix_shapes(args, args.sm_count):
+            print(json.dumps(cfg))
+        return
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_decode.py needs a CUDA device (use --dry-run without one)")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    name, power, clock = card_settings()
+    sm = torch.cuda.get_device_properties(dev).multi_processor_count
+    hq, hkv, d = args.hq, args.hkv, args.head_dim
+    fp8 = args.kv_dtype == "e4m3"
+    for cfg in prefix_shapes(args, sm):
+        n_prompts, length, n, b, suf = cfg["prompts"], cfg["shared_prefix"], cfg["samples"], cfg["batch"], cfg["suffix"]
+        torch.manual_seed(0)
+        q = torch.randn(b, 1, hq, d, device=dev, dtype=torch.bfloat16)
+        k_new, v_new = (torch.randn(b, 1, hkv, d, device=dev, dtype=torch.bfloat16) for _ in range(2))
+        pk, pv = (torch.randn(n_prompts, length, hkv, d, device=dev, dtype=torch.bfloat16) for _ in range(2))
+        sk, sv = (torch.randn(b, suf, hkv, d, device=dev, dtype=torch.bfloat16) for _ in range(2))
+        kw, pkw = {}, {}
+        if fp8:  # one descale per kv head for prompt and samples alike, so that every arm holds the same contents
+            kd = torch.maximum(pk.abs().amax(dim=(0, 1, 3)), sk.abs().amax(dim=(0, 1, 3))).float() / 448
+            vd = torch.maximum(pv.abs().amax(dim=(0, 1, 3)), sv.abs().amax(dim=(0, 1, 3))).float() / 448
+            pk, sk = (torch.stack([dec.quantize_e4m3(x[i], kd) for i in range(x.shape[0])]) for x in (pk, sk))
+            pv, sv = (torch.stack([dec.quantize_e4m3(x[i], vd) for i in range(x.shape[0])]) for x in (pv, sv))
+            kw = dict(k_descale=kd.expand(b, hkv).contiguous(), v_descale=vd.expand(b, hkv).contiguous())
+            pkw = dict(prefix_k_descale=kd.expand(n_prompts, hkv).contiguous(),
+                       prefix_v_descale=vd.expand(n_prompts, hkv).contiguous())
+        scale = d ** -0.5
+        # every call appends one token at the same row (the last of the suffix), so each arm repeats the same step
+        sl_own = torch.full((b,), suf - 1, dtype=torch.int32, device=dev)
+        sl_all = sl_own + length
+        pl = torch.full((n_prompts,), length, dtype=torch.int32, device=dev)
+        owner = torch.arange(b, device=dev) // n
+
+        def raw(x):
+            return x.view(torch.uint8)
+
+        # copied: the prompt ahead of each sample's suffix in one contiguous cache
+        ck = torch.cat([raw(pk)[owner], raw(sk)], dim=1).view(pk.dtype)
+        cv = torch.cat([raw(pv)[owner], raw(sv)], dim=1).view(pv.dtype)
+        # paged: the prompt's pages once per prompt, then each sample's own pages; the tables share the prompt pages
+        p_pages, s_pages = -(-length // PREFIX_PAGE), -(-suf // PREFIX_PAGE)
+        assert length % PREFIX_PAGE == 0, "--shared-prefix must be a multiple of 128 for the paged arm"
+
+        def pool_of(pre, own):
+            rb = d * pre.element_size()  # bytes per (row, kv head)
+            pool = torch.zeros((n_prompts * p_pages + b * s_pages, PREFIX_PAGE, hkv, rb), dtype=torch.uint8,
+                               device=dev)
+            pool[:n_prompts * p_pages] = raw(pre).reshape(n_prompts * p_pages, PREFIX_PAGE, hkv, rb)
+            padded = torch.zeros((b, s_pages * PREFIX_PAGE, hkv, rb), dtype=torch.uint8, device=dev)
+            padded[:, :suf] = raw(own)
+            pool[n_prompts * p_pages:] = padded.view(b * s_pages, PREFIX_PAGE, hkv, rb)
+            return pool.view(pre.dtype)
+
+        gk, gv = pool_of(pk, sk), pool_of(pv, sv)
+        table = torch.cat([owner[:, None] * p_pages + torch.arange(p_pages, device=dev)[None],
+                           n_prompts * p_pages + torch.arange(b * s_pages, device=dev).view(b, s_pages)],
+                          dim=1).to(torch.int32)
+
+        def prefix_call():
+            return dec.kernel_decode(q, sk, sv, sl_own, k_new, v_new, True, scale, prefix_k_cache=pk,
+                                     prefix_v_cache=pv, prefix_seqlens=pl, **kw, **pkw)
+
+        def copied_call():
+            return dec.kernel_decode(q, ck, cv, sl_all, k_new, v_new, True, scale, **kw)
+
+        def paged_call():
+            return dec.kernel_decode(q, gk, gv, sl_all, k_new, v_new, True, scale, block_table=table, **kw)
+
+        arms = {"prefix": prefix_call, "copied": copied_call, "paged": paged_call}
+        times = {k: [] for k in arms}
+        for _ in range(5):  # alternate them in one run
+            for k, fn in arms.items():
+                times[k].append(time_us(fn, args.iters, args.warmup))
+        res = dict(cfg, card=name, power_limit=power, max_sm_clock=clock)
+        for k, ts in times.items():
+            us = min(ts)
+            res[f"{k}_us"] = round(us, 2)
+            res[f"{k}_us_all"] = [round(t, 2) for t in ts]
+            res[f"{k}_GBps"] = round(cfg[f"{k}_bytes"] / (us * 1e-6) / 1e9, 1)
+        res["prefix_speedup_vs_copied"] = round(res["copied_us"] / res["prefix_us"], 3)
+        res["prefix_speedup_vs_paged"] = round(res["paged_us"] / res["prefix_us"], 3)
+        outs = {k: fn()[0].float() for k, fn in arms.items()}
+        res["max_abs_diff_prefix_vs_copied"] = (outs["prefix"] - outs["copied"]).abs().max().item()
+        res["max_abs_diff_paged_vs_copied"] = (outs["paged"] - outs["copied"]).abs().max().item()
+        print(json.dumps(res), flush=True)
+        del q, k_new, v_new, pk, pv, sk, sv, ck, cv, gk, gv, outs
+        torch.cuda.empty_cache()
+
+
 def card():
     name = torch.cuda.get_device_name(0)
     try:
@@ -158,6 +300,9 @@ def time_us(fn, iters, warmup):
 
 def main():
     args = parse_args()
+    if args.shared_prefix is not None:
+        shared_prefix_main(args)
+        return
     if args.dry_run:
         for cfg in shapes(args, args.sm_count):
             print(json.dumps(cfg))

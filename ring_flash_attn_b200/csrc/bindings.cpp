@@ -591,6 +591,124 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
                                at::cuda::getCurrentCUDAStream()));
 }
 
+// The shared-prefix pass of split-KV decode (see decode_prefix_launch): attention of q (B, Sq, Hq, D), or varlen
+// (total_q, Hq, D) with cu_seqlens_q (B + 1,), to P shared prefixes prefix_k / prefix_v (P, P_cap, Hkv, D) with
+// mergeable first two dimensions, in q's dtype or both e4m3 with k_descale / v_descale fp32 (P, Hkv) contiguous.
+// Sequence b reads prefix b / (B / P), rows [0, prefix_seqlens[p]) (read on the device only, clamped to [0, P_cap]),
+// all visible to every query token.  part: the partial slabs of this pass, in decode_fwd's layout.  causal and the
+// rotary tensors position q's rotation as in decode_fwd.
+void decode_prefix_fwd(const at::Tensor& q_in, const at::Tensor& prefix_k, const at::Tensor& prefix_v,
+                       const at::Tensor& prefix_seqlens, bool causal, double scale, at::Tensor& part,
+                       const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale,
+                       const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q,
+                       const c10::optional<at::Tensor>& rotary_cos, const c10::optional<at::Tensor>& rotary_sin,
+                       const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved) {
+  const c10::cuda::CUDAGuard guard(q_in.device());
+  const bool varlen = cu_seqlens_q.has_value();
+  TORCH_CHECK(q_in.dim() == (varlen ? 3 : 4), "decode_prefix_fwd: q must be (B, Sq, Hq, D), or (total_q, Hq, D) "
+              "with cu_seqlens_q");
+  TORCH_CHECK(q_in.scalar_type() == at::kBFloat16 || q_in.scalar_type() == at::kHalf,
+              "decode_prefix_fwd: q must be bf16 or fp16");
+  const int64_t total_q = varlen ? q_in.size(0) : 0;
+  if (varlen) {
+    const at::Tensor& cu = *cu_seqlens_q;
+    TORCH_CHECK(cu.scalar_type() == at::kInt && cu.device() == q_in.device() && cu.is_contiguous() && cu.dim() == 1 &&
+                    cu.numel() >= 2,
+                "decode_prefix_fwd: cu_seqlens_q must be (B + 1,) int32 contiguous on q's device");
+    TORCH_CHECK(max_seqlen_q >= 1, "decode_prefix_fwd: max_seqlen_q must be >= 1");
+  }
+  const at::Tensor q = varlen ? q_in.unsqueeze(0) : q_in;
+  const int64_t B = varlen ? cu_seqlens_q->numel() - 1 : q.size(0);
+  const int64_t sq = varlen ? max_seqlen_q : q.size(1), hq = q.size(2), d = q.size(3);
+  const int64_t rows = varlen ? total_q : B * sq;
+  TORCH_CHECK(prefix_k.dim() == 4 && prefix_k.sizes() == prefix_v.sizes(),
+              "decode_prefix_fwd: prefix_k / prefix_v must be the same (P, P_cap, Hkv, D) shape");
+  const int64_t n_prefix = prefix_k.size(0), p_cap = prefix_k.size(1), hkv = prefix_k.size(2);
+  const bool fp8 = prefix_k.scalar_type() == at::kFloat8_e4m3fn;
+  TORCH_CHECK(prefix_k.scalar_type() == prefix_v.scalar_type() && (fp8 || prefix_k.scalar_type() == q.scalar_type()),
+              "decode_prefix_fwd: the prefix caches must both have q's dtype or both be fp8 (float8_e4m3fn)");
+  TORCH_CHECK(k_descale.has_value() == fp8 && v_descale.has_value() == fp8,
+              "decode_prefix_fwd: fp8 prefix caches need k_descale and v_descale, and other caches take none");
+  TORCH_CHECK(n_prefix >= 1 && B % n_prefix == 0 && prefix_k.size(3) == d && hkv >= 1 && hq % hkv == 0,
+              "decode_prefix_fwd: the prefix caches do not match q (P must divide B)");
+  TORCH_CHECK(n_prefix * p_cap < (int64_t(1) << 31), "decode_prefix_fwd: P * P_cap must be below 2^31");
+  TORCH_CHECK(q.stride(3) == 1 && (varlen || q.stride(0) == sq * q.stride(1)),
+              "decode_prefix_fwd: q must be (B, Sq) mergeable");
+  TORCH_CHECK((q.stride(1) * q.element_size()) % 16 == 0 && (q.stride(2) * q.element_size()) % 16 == 0 &&
+                  reinterpret_cast<uintptr_t>(q.data_ptr()) % 16 == 0,
+              "decode_prefix_fwd: q rows must be 16-byte aligned");
+  for (const at::Tensor* c : {&prefix_k, &prefix_v})
+    TORCH_CHECK(c->device() == q.device() && c->stride(3) == 1 && c->stride(0) == c->size(1) * c->stride(1),
+                "decode_prefix_fwd: the prefix caches must be on q's device with mergeable first two dimensions");
+  TORCH_CHECK(prefix_seqlens.scalar_type() == at::kInt && prefix_seqlens.device() == q.device() &&
+                  prefix_seqlens.is_contiguous() && prefix_seqlens.dim() == 1 && prefix_seqlens.numel() == n_prefix,
+              "decode_prefix_fwd: prefix_seqlens must be (P,) int32 contiguous on q's device");
+  TORCH_CHECK(part.scalar_type() == at::kFloat && part.dim() == 2 && part.size(0) >= 1 && part.stride(1) == 1 &&
+                  part.size(1) == rows * hq * d + rows * hq && part.stride(0) >= part.size(1) &&
+                  part.stride(0) % 2 == 0 && reinterpret_cast<uintptr_t>(part.data_ptr()) % 8 == 0,
+              "decode_prefix_fwd: part must be fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq), or total_q for B*Sq when "
+              "varlen, with stride(1) == 1, an even stride(0) and an 8-byte aligned start");
+  const int64_t n_splits = part.size(0);
+  const int64_t tiles = (p_cap + 127) / 128;
+  rfa::DecodeParams p{};
+  p.q = q.data_ptr();
+  p.q_row_stride = q.stride(1);
+  p.q_head_stride = q.stride(2);
+  p.seqlens = prefix_seqlens.data_ptr<int>();
+  p.part = part.data_ptr<float>();
+  p.part_stride = part.stride(0);
+  p.batch = static_cast<int>(B);
+  p.sq = static_cast<int>(sq);
+  p.hq = static_cast<int>(hq);
+  p.hkv = static_cast<int>(hkv);
+  p.cu_seqlens_q = varlen ? cu_seqlens_q->data_ptr<int>() : nullptr;
+  p.total_q = static_cast<int>(rows);
+  p.s_cap = static_cast<int>(p_cap);
+  p.tiles_per_split = static_cast<int>(std::max<int64_t>(1, (tiles + n_splits - 1) / n_splits));
+  p.n_new = 0;
+  p.causal = causal ? 1 : 0;
+  p.scale_log2 = static_cast<float>(scale * 1.4426950408889634);
+  p.prefix_n = static_cast<int>(B / n_prefix);
+  if (fp8) {
+    for (const at::Tensor* t : {&*k_descale, &*v_descale})
+      TORCH_CHECK(t->scalar_type() == at::kFloat && t->device() == q.device() && t->dim() == 2 &&
+                      t->size(0) == n_prefix && t->size(1) == hkv && t->is_contiguous(),
+                  "decode_prefix_fwd: fp8 descales must be contiguous fp32 (P, Hkv) on q's device");
+    p.k_descale = k_descale->data_ptr<float>();
+    p.v_descale = v_descale->data_ptr<float>();
+  }
+  TORCH_CHECK(rotary_cos.has_value() == rotary_sin.has_value() && rotary_cos.has_value() == rotary_seqlens.has_value(),
+              "decode_prefix_fwd: rotary needs rotary_cos, rotary_sin and rotary_seqlens together");
+  if (rotary_cos.has_value()) {
+    const at::Tensor& rc = *rotary_cos;
+    const at::Tensor& rs = *rotary_sin;
+    TORCH_CHECK(rc.dim() == 2 && rc.sizes() == rs.sizes() && rc.size(0) >= 1 && rc.is_contiguous() &&
+                    rs.is_contiguous() && rc.scalar_type() == q.scalar_type() &&
+                    rs.scalar_type() == q.scalar_type() && rc.device() == q.device() && rs.device() == q.device(),
+                "decode_prefix_fwd: rotary_cos / rotary_sin must be contiguous (seqlen_ro, rotary_dim / 2) in q's "
+                "dtype on q's device");
+    TORCH_CHECK(rc.size(1) >= 8 && rc.size(1) % 8 == 0 && 2 * rc.size(1) <= d,
+                "decode_prefix_fwd: rotary_dim must be a positive multiple of 16, at most head_dim");
+    TORCH_CHECK(rc.size(0) < (int64_t(1) << 31), "decode_prefix_fwd: seqlen_ro must be below 2^31");
+    const at::Tensor& rsl = *rotary_seqlens;
+    TORCH_CHECK(rsl.scalar_type() == at::kInt && rsl.device() == q.device() && rsl.is_contiguous() && rsl.dim() == 1 &&
+                    rsl.numel() == B,
+                "decode_prefix_fwd: rotary_seqlens must be (B,) int32 contiguous on q's device");
+    p.rotary_cos = rc.data_ptr();
+    p.rotary_sin = rs.data_ptr();
+    p.rotary_seqlens = rsl.data_ptr<int>();
+    p.rotary_half = static_cast<int>(rc.size(1));
+    p.seqlen_ro = static_cast<int>(rc.size(0));
+    p.rotary_interleaved = rotary_interleaved ? 1 : 0;
+  }
+  const int64_t cache_rows = n_prefix * p_cap;
+  const TensorView kv{prefix_k.data_ptr(), cache_rows, static_cast<int>(hkv), prefix_k.stride(1), prefix_k.stride(2)};
+  const TensorView vv{prefix_v.data_ptr(), cache_rows, static_cast<int>(hkv), prefix_v.stride(1), prefix_v.stride(2)};
+  check(rfa::decode_prefix_launch(dtype_code(q), fp8 ? rfa::kDtypeE4M3 : dtype_code(q), kv, vv, p,
+                                  static_cast<int>(n_prefix), static_cast<int>(n_splits), static_cast<int>(d),
+                                  at::cuda::getCurrentCUDAStream()));
+}
+
 // Merges the partials of decode_fwd (or gathered per-rank partials, same layout): out (B, Sq, Hq, D) contiguous in
 // bf16 / fp16 / fp32, lse (B, Hq, Sq) fp32 contiguous.
 void decode_combine(const at::Tensor& parts, at::Tensor& out, at::Tensor& lse) {
@@ -681,6 +799,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                cu_seqlens_q, max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, c10::nullopt,
                c10::nullopt, c10::nullopt);
   });
+  m.def("decode_prefix_fwd", &decode_prefix_fwd);
   m.def("decode_combine", &decode_combine);
   rfa::bind_peer_mem(m);
 }

@@ -57,6 +57,9 @@ struct DecodeParams {
   const int* cache_batch_idx;  // (B,)
   int cache_batch;
   const int* cache_leftpad;  // (B,)
+  // Shared prefixes (decode_prefix_launch only): sequences [i * prefix_n, (i + 1) * prefix_n) share prefix i, whose
+  // valid rows are seqlens[i] (clamped to [0, s_cap]) of a (P, s_cap, Hkv, D) cache; the descales are (P, Hkv).
+  int prefix_n;
 };
 
 // Appends k_new / v_new (B, Sq, Hkv, D), contiguous, in q's dtype, at rows [seqlens[b], seqlens[b] + Sq) of the
@@ -72,6 +75,22 @@ struct DecodeParams {
 const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_cache, const TensorView& v_cache,
                               const void* k_new, const void* v_new, int new_dtype, const DecodeParams& p,
                               int n_splits, int head_dim, cudaStream_t stream);
+
+// The shared-prefix pass: attention of every query row to its group's prefix, into the partial slabs of `p.part`
+// (the same layout as decode_fwd_launch's; a caller merges both passes' slabs with one decode_combine_launch).  The
+// caches k_prefix / v_prefix are (n_prefix, p.s_cap, Hkv, D) with mergeable first two dimensions; p.seqlens are the
+// prefixes' valid rows, p.k_descale / p.v_descale (n_prefix, Hkv) with e4m3 caches, p.prefix_n = B / n_prefix.
+// Every prefix key is visible to every query token (p.n_new must be 0); q is rotated as in decode_fwd_launch.  No
+// append, block table, cache slots, left pads or e4m3 q.  The grid is (n_splits, decode_prefix_slots(p), n_prefix *
+// Hkv): a CTA takes 64 consecutive packed rows of one group, rows [b0 * sq, (b0 + n) * sq) of a uniform q or
+// [cu[b0], cu[b0 + n]) of a varlen one (b0 = prefix * n), each row (sequence, token, head-in-group) in that order.
+const char* decode_prefix_launch(int dtype, int cache_dtype, const TensorView& k_prefix, const TensorView& v_prefix,
+                                 const DecodeParams& p, int n_prefix, int n_splits, int head_dim,
+                                 cudaStream_t stream);
+
+// Row-tile slots per (split, prefix, kv head) of the shared-prefix pass, from shapes only: ceil(rows * G / 64) for a
+// group's rows, n * sq (uniform) or min(n * sq, total_q) (varlen, sq = max_seqlen_q).
+long long decode_prefix_slots(const DecodeParams& p);
 
 // Varlen row-tile slots, from shapes only: min(B * ceil(sq * G / 64), (total_q * G + 63 * B) / 64), an upper bound
 // on sum_b ceil(n_b * G / 64) for any counts n_b <= sq that sum to total_q.

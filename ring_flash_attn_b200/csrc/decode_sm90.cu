@@ -47,6 +47,14 @@
 // slot shifted down by lp rows.  Only the producer's row coordinate (slot * S_cap + lp + key) and the append's target
 // row see the slot and the pad.  Tile rows past the last visible key may reach into the next slot or past the tensor
 // (TMA fills those with zeros); they are discarded like any row at or past the limit.
+//
+// Shared prefixes (kPrefix, decode_prefix_launch): the n = B / P consecutive sequences of group i share prefix i, a
+// (P, P_cap, Hkv, D) cache read by a second pass.  Its grid is (prefix split, row-tile slot, P x Hkv): a CTA takes 64
+// consecutive packed rows of the group's (sequence, token, head-in-group) rows, which are rows [b0 * sq, (b0 + n) *
+// sq) of a uniform q or [cu[b0], cu[b0 + n]) of a varlen one, so the group's samples share each prefix K / V tile.
+// Everything runs as a call with cache slot i, seqlens[i] valid rows, no append (every prefix key is visible to every
+// row) and descales [i, kv head]; only the rotary position and the lse address need a row's own sequence and token.
+// Its partials go to slabs after the suffix pass's, and the one combine merges both.
 #include <math_constants.h>
 
 #include <type_traits>
@@ -207,6 +215,33 @@ __device__ __forceinline__ bool varlen_tile(const DecodeParams& p, int slot, int
   return false;
 }
 
+// Shared-prefix pass: the group of sequences [b0, b0 + prefix_n): its first packed query row (x) and row count (y),
+// clamped like q_rows, so rows [x, x + y) always lie inside q and the partial buffer.
+__device__ __forceinline__ int2 prefix_rows(const DecodeParams& p, int b0) {
+  if (p.cu_seqlens_q == nullptr) return make_int2(b0 * p.sq, p.prefix_n * p.sq);
+  const int lo = clamp_to(__ldg(p.cu_seqlens_q + b0), 0, p.total_q);
+  const int hi = clamp_to(__ldg(p.cu_seqlens_q + b0 + p.prefix_n), 0, p.total_q);
+  return make_int2(lo, hi > lo ? hi - lo : 0);
+}
+
+// The sequence b and token t of packed query row `row` of the group starting at sequence b0: the last sequence of the
+// group whose first row is at or before `row` (a binary search over cu when varlen).
+__device__ __forceinline__ void prefix_token(const DecodeParams& p, int b0, int row, int& b, int& t) {
+  if (p.cu_seqlens_q == nullptr) {
+    b = row / p.sq;
+    t = row - b * p.sq;
+    return;
+  }
+  int lo = b0, hi = b0 + p.prefix_n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (clamp_to(__ldg(p.cu_seqlens_q + mid), 0, p.total_q) <= row) lo = mid;
+    else hi = mid - 1;
+  }
+  b = lo;
+  t = row - clamp_to(__ldg(p.cu_seqlens_q + lo), 0, p.total_q);
+}
+
 // TMA producer over a paged cache, run by the whole producer warp.  A 128-key tile is one page (page_size >= 128,
 // the tile starts at row key0 % page_size of it) or 128 / page_size pages, each loaded as its own box of page_size
 // rows into the matching rows of the slot: an offset of i * page_size * 128 bytes stays 1024-byte aligned, so the
@@ -315,13 +350,14 @@ __device__ __forceinline__ uint64_t f8_desc(const uint8_t* tile) {
   return kD == 128 ? gmma_desc(smem_u32(tile), 0) : gmma_desc_sw64(smem_u32(tile));
 }
 
-// kQ8: e4m3 queries (T = bf16, kFp8 set), see the file comment.
-template <typename T, int kD, bool kFp8, bool kQ8>
+// kQ8: e4m3 queries (T = bf16, kFp8 set); kPrefix: the shared-prefix pass.  See the file comment.
+template <typename T, int kD, bool kFp8, bool kQ8, bool kPrefix = false>
 __global__ void __launch_bounds__(kFp8 ? kThreadsFp8 : kThreads, 1)
 decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
               const __grid_constant__ DecodeParams p) {
   static_assert(kD == 64 || kD == 128, "head dim 64 or 128");
   static_assert(!kQ8 || (kFp8 && std::is_same_v<T, __nv_bfloat16>), "e4m3 queries: e4m3 cache, bf16 P V");
+  static_assert(!(kPrefix && kQ8), "a shared prefix takes a bf16 / fp16 q");
   using L = LoadRing<kD, kFp8, kQ8>;
   constexpr int kSubTiles = kD / 64;
   // T slots the compute warpgroup reads
@@ -332,8 +368,14 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   const int split = blockIdx.x;
   const int group = p.hq / p.hkv;
   int b, kv_head, row0;
-  int2 qr;  // the sequence's first packed query row and token count
-  if (p.cu_seqlens_q == nullptr) {
+  int2 qr;  // the sequence's first packed query row and token count (kPrefix: the group's)
+  if constexpr (kPrefix) {  // b is the prefix: it indexes seqlens, the cache slot and the descales
+    b = blockIdx.z / p.hkv;
+    kv_head = blockIdx.z % p.hkv;
+    qr = prefix_rows(p, b * p.prefix_n);
+    row0 = blockIdx.y * kRows;
+    if (row0 >= qr.y * group) return;  // an idle slot, in every role: nothing to write
+  } else if (p.cu_seqlens_q == nullptr) {
     b = blockIdx.z / p.hkv;
     kv_head = blockIdx.z % p.hkv;
     row0 = blockIdx.y * kRows;
@@ -394,7 +436,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
 
   if (threadIdx.x >= kProducer) {
     // ------------------------------------------------------------------ TMA producer
-    if (p.page_size != 0) {
+    if (!kPrefix && p.page_size != 0) {
       if (n_tiles > 0)
         produce_paged<kD, kFp8, kQ8>(&tm_k, &tm_v, load_full, load_empty, smem_load, p, b, kv_head, j0, n_tiles,
                                      kmax);
@@ -510,8 +552,11 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
         const int t = pr / group, head = kv_head * group + pr % group;
         const T* q_row = q + static_cast<long long>(qr.x + t) * p.q_row_stride + head * p.q_head_stride;
         val = *reinterpret_cast<const uint4*>(q_row + 8 * c);
-        if (p.rotary_cos != nullptr && c < p.rotary_half / 4)
-          val = rotate_chunk<T>(val, q_row, c, rotary_pos(p, b, p.causal ? t : 0), p);
+        if (p.rotary_cos != nullptr && c < p.rotary_half / 4) {
+          int rb = b, rt = t;  // the row's own sequence and token
+          if constexpr (kPrefix) prefix_token(p, b * p.prefix_n, qr.x + t, rb, rt);
+          val = rotate_chunk<T>(val, q_row, c, rotary_pos(p, rb, p.causal ? rt : 0), p);
+        }
       }
       *reinterpret_cast<uint4*>(smem_q + (c >> 3) * kQHalfBytes + r * 128 + (((c & 7) ^ (r & 7)) << 4)) = val;
     }
@@ -702,7 +747,15 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
           make_float2(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
     if ((lane & 3) == 0) {
       const float lse = lt > 0.f ? (m2[h] + __log2f(lt)) * 0.6931471805599453f : -CUDART_INF_F;
-      lse_row[static_cast<long long>(head) * lse_stride + t] = lse;
+      if constexpr (kPrefix) {
+        // packed row qr.x + t: lse at (head, row) varlen, at (b, head, t) of row = b * sq + t uniform
+        const int row = qr.x + t;
+        const long long li = varlen ? static_cast<long long>(head) * p.total_q + row
+                                    : (static_cast<long long>(row / p.sq) * p.hq + head) * p.sq + row % p.sq;
+        part[n_out * kD + li] = lse;
+      } else {
+        lse_row[static_cast<long long>(head) * lse_stride + t] = lse;
+      }
     }
   }
 }
@@ -937,6 +990,71 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
   if (err != cudaSuccess) return cudaGetErrorString(err);
   err = cudaGetLastError();
   return err == cudaSuccess ? nullptr : cudaGetErrorString(err);
+}
+
+const char* decode_prefix_launch(int dtype, int cache_dtype, const TensorView& k_prefix, const TensorView& v_prefix,
+                                 const DecodeParams& p, int n_prefix, int n_splits, int head_dim,
+                                 cudaStream_t stream) {
+  if (head_dim != 64 && head_dim != 128) return "the sm_90a decode kernel is instantiated for head_dim 64 and 128";
+  if (dtype != kDtypeBF16 && dtype != kDtypeFP16) return "a shared prefix takes a bf16 / fp16 q";
+  const bool fp8 = cache_dtype == kDtypeE4M3;
+  if (!fp8 && cache_dtype != dtype) return "the prefix caches must have q's dtype or be e4m3";
+  if (fp8 != (p.k_descale != nullptr && p.v_descale != nullptr))
+    return "e4m3 prefix caches need k / v descales, and only e4m3 caches take them";
+  if (p.q_descale != nullptr || p.n_new != 0 || p.page_size != 0 || p.cache_batch_idx != nullptr ||
+      p.cache_leftpad != nullptr)
+    return "the shared-prefix pass takes no q_descale, append, block table, cache slots or left pads";
+  if (p.hkv <= 0 || p.hq % p.hkv != 0) return "query heads must be a multiple of kv heads";
+  if (n_prefix < 1 || p.batch % n_prefix != 0 || p.prefix_n != p.batch / n_prefix)
+    return "the batch must be prefix_n sequences per prefix";
+  if (k_prefix.row_stride != v_prefix.row_stride || k_prefix.head_stride != v_prefix.head_stride)
+    return "the prefix caches must have the same strides";
+  if (p.rotary_cos != nullptr) {
+    if (p.rotary_sin == nullptr || p.rotary_seqlens == nullptr) return "rotary needs cos, sin and rotary_seqlens";
+    if (p.rotary_half <= 0 || p.rotary_half % 8 != 0 || 2 * p.rotary_half > head_dim)
+      return "rotary_dim must be a positive multiple of 16, at most head_dim";
+    if (p.seqlen_ro < 1) return "the rotary tables must have at least one row";
+  }
+  const long long slots = decode_prefix_slots(p);
+  if (slots > 65535) return "shared prefix: more than 65535 row tiles per group";
+  if (static_cast<long long>(n_prefix) * p.hkv > 65535) return "shared prefix: more than 65535 (prefix, kv head) pairs";
+  if (slots == 0) return nullptr;  // no query rows
+  const int elem_bytes = fp8 ? 1 : 2;
+  const int swizzle = fp8 ? head_dim : 128;
+  CUtensorMap tk, tv;
+  if (const char* e = make_tensor_map(&tk, k_prefix, elem_bytes, dec::kTile, head_dim, swizzle)) return e;
+  if (const char* e = make_tensor_map(&tv, v_prefix, elem_bytes, dec::kTile, head_dim, swizzle)) return e;
+  const dim3 grid(n_splits, static_cast<unsigned>(slots), n_prefix * p.hkv);
+  cudaError_t err = cudaSuccess;
+  auto launch = [&](auto kern, int smem, int threads) {
+    err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (err == cudaSuccess) kern<<<grid, threads, smem, stream>>>(tk, tv, p);
+  };
+  auto pick = [&](auto t, auto f8) {
+    using T = decltype(t);
+    constexpr bool kFp8 = decltype(f8)::value;
+    const int threads = kFp8 ? dec::kThreadsFp8 : dec::kThreads;
+    if (head_dim == 128)
+      launch(dec::decode_kernel<T, 128, kFp8, false, true>, dec::smem_bytes<128, kFp8, false>(), threads);
+    else launch(dec::decode_kernel<T, 64, kFp8, false, true>, dec::smem_bytes<64, kFp8, false>(), threads);
+  };
+  if (dtype == kDtypeBF16) {
+    if (fp8) pick(__nv_bfloat16{}, std::true_type{});
+    else pick(__nv_bfloat16{}, std::false_type{});
+  } else {
+    if (fp8) pick(__half{}, std::true_type{});
+    else pick(__half{}, std::false_type{});
+  }
+  if (err != cudaSuccess) return cudaGetErrorString(err);
+  err = cudaGetLastError();
+  return err == cudaSuccess ? nullptr : cudaGetErrorString(err);
+}
+
+long long decode_prefix_slots(const DecodeParams& p) {
+  const long long group = p.hq / p.hkv;
+  long long rows = static_cast<long long>(p.prefix_n) * p.sq;
+  if (p.cu_seqlens_q != nullptr && p.total_q < rows) rows = p.total_q;
+  return (rows * group + dec::kRows - 1) / dec::kRows;
 }
 
 long long decode_tile_slots(const DecodeParams& p) {

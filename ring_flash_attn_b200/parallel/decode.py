@@ -70,6 +70,22 @@ def num_splits_varlen(batch: int, total_q: int, max_seqlen_q: int, hq: int, hkv:
     return max(1, min(tiles, sm_count // (slots * hkv)))
 
 
+def prefix_tile_slots(n: int, sq: int, hq: int, hkv: int, total_q: Optional[int] = None) -> int:
+    """Row-tile slots of the shared-prefix pass per (prefix, kv head): ``ceil(rows * G / 64)`` for the ``rows`` of
+    one group of ``n`` sequences, ``n * sq``, or ``min(n * max_seqlen_q, total_q)`` for a varlen call.  From shapes
+    only; slots past a group's last real tile exit at once."""
+    rows = n * sq if total_q is None else min(n * sq, total_q)
+    return -(-rows * (hq // hkv) // ROWS_PER_CTA)
+
+
+def num_splits_prefix(n_prefix: int, slots: int, hkv: int, p_cap: int, sm_count: int) -> int:
+    """Key-range splits of the shared-prefix pass: :func:`num_splits` with ``P`` prefixes of ``slots`` row tiles
+    (:func:`prefix_tile_slots`) for the ``B`` sequences, and ``P_cap`` for ``S_cap``.  One full wave, from shapes
+    only, never from ``prefix_seqlens``."""
+    tiles = max(1, -(-p_cap // KEY_TILE))
+    return max(1, min(tiles, sm_count // (n_prefix * hkv * max(1, slots))))
+
+
 _warned = set()
 
 
@@ -116,7 +132,10 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
                   rotary_cos: Optional[Tensor] = None, rotary_sin: Optional[Tensor] = None,
                   rotary_seqlens: Optional[Tensor] = None, rotary_interleaved: bool = True,
                   q_descale: Optional[Tensor] = None, cache_batch_idx: Optional[Tensor] = None,
-                  cache_leftpad: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+                  cache_leftpad: Optional[Tensor] = None, prefix_k_cache: Optional[Tensor] = None,
+                  prefix_v_cache: Optional[Tensor] = None, prefix_seqlens: Optional[Tensor] = None,
+                  prefix_k_descale: Optional[Tensor] = None, prefix_v_descale: Optional[Tensor] = None,
+                  prefix_splits: Optional[int] = None) -> Tuple[Tensor, Tensor]:
     """Local split-KV kernel (appending ``k`` / ``v`` first when given), then the combine over the splits and, for
     ``world > 1``, over the gathered per-rank partials.  ``splits`` overrides :func:`num_splits`.  With
     ``block_table`` the caches are page pools (see :func:`cp_flash_attn_with_kvcache`).  e4m3 caches take contiguous
@@ -126,7 +145,11 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
     and ``k`` before it stores it, as :func:`apply_rotary` does, at positions clamped to the tables.  An e4m3 ``q``
     (over e4m3 caches) takes a contiguous fp32 ``(B, Hkv)`` ``q_descale`` and gives a bf16 ``out``; e4m3 ``k`` / ``v``
     over e4m3 caches are stored as they are.  ``cache_batch_idx`` / ``cache_leftpad`` (contiguous ``(B,)`` int32,
-    contiguous caches only) select each sequence's cache slot and first key row, read on the device only."""
+    contiguous caches only) select each sequence's cache slot and first key row, read on the device only.  With
+    ``prefix_k_cache`` / ``prefix_v_cache`` ``(P, P_cap, Hkv, D)`` (contiguous), ``prefix_seqlens`` ``(P,)`` int32 and,
+    for e4m3 caches, contiguous fp32 ``(P, Hkv)`` ``prefix_k_descale`` / ``prefix_v_descale``, a second kernel adds
+    the attention of sequence ``b`` to prefix ``b // (B // P)``, in ``prefix_splits`` (default
+    :func:`num_splits_prefix`) more partial slabs that the same combine merges."""
     C = cuda_ext.load()
     varlen = cu_seqlens_q is not None
     if varlen:  # the partials are the uniform layout at batch 1, Sq = total_q
@@ -146,18 +169,31 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
             splits = num_splits_varlen(b, total_q, max_seqlen_q, hq, hkv, s_cap, _sm_count(dev))
         else:
             splits = num_splits(b, sq, hq, hkv, s_cap, _sm_count(dev))
+    prefix = prefix_k_cache is not None
+    if prefix and prefix_splits is None:
+        dev = q.device.index if q.device.index is not None else torch.cuda.current_device()
+        n_prefix, hkv = prefix_k_cache.shape[0], prefix_k_cache.shape[2]
+        slots = prefix_tile_slots(b // n_prefix, max_seqlen_q if varlen else sq, hq, hkv,
+                                  total_q if varlen else None)
+        prefix_splits = num_splits_prefix(n_prefix, slots, hkv, prefix_k_cache.shape[1], _sm_count(dev))
+    n_slabs = splits + (prefix_splits if prefix else 0)
     n_out = rows_b * rows_sq * hq * d
     size = n_out + rows_b * hq * rows_sq
     # every split's partial starts 8-byte aligned (the kernel stores out as float2): rows * Hq * (D + 1) is odd when
     # rows and Hq are
-    parts = torch.empty((splits, size + size % 2), dtype=torch.float32, device=q.device)[:, :size]
+    parts = torch.empty((n_slabs, size + size % 2), dtype=torch.float32, device=q.device)[:, :size]
     extra = () if q_descale is None else (q_descale,)  # decode_fwd takes q_descale only for an e4m3 q
     if cache_batch_idx is not None or cache_leftpad is not None:
         extra = (q_descale, cache_batch_idx, cache_leftpad)
-    C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts, block_table, k_descale,
-                 v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0, rotary_cos, rotary_sin, rotary_seqlens,
-                 bool(rotary_interleaved), *extra)
+    C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts[:splits], block_table,
+                 k_descale, v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0, rotary_cos, rotary_sin,
+                 rotary_seqlens, bool(rotary_interleaved), *extra)
     cuda_ext.note_launch(2 if k is not None else 1)
+    if prefix:  # the prefix partials go to the slabs after the suffix pass's
+        C.decode_prefix_fwd(q, prefix_k_cache, prefix_v_cache, prefix_seqlens, causal, softmax_scale, parts[splits:],
+                            prefix_k_descale, prefix_v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0,
+                            rotary_cos, rotary_sin, rotary_seqlens, bool(rotary_interleaved))
+        cuda_ext.note_launch()
     if world > 1:
         mine = torch.empty(size, dtype=torch.float32, device=q.device)
         C.decode_combine(parts, mine[:n_out].view(rows_b, rows_sq, hq, d), mine[n_out:].view(rows_b, hq, rows_sq))
@@ -229,7 +265,7 @@ def _varlen_spans(cu_seqlens_q: Tensor, total_q: int, max_seqlen_q: int):
 
 def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table=None,
                   k_descale=None, v_descale=None, cu_seqlens_q=None, max_seqlen_q=0, rotary=None, q_descale=None,
-                  cache_batch_idx=None, cache_leftpad=None):
+                  cache_batch_idx=None, cache_leftpad=None, prefix=None):
     # every sequence is a (first row, count) span of the packed rows: (b * Sq, Sq) for a uniform q
     out_dtype = _out_dtype(q)
     b = cache_seqlens.shape[0]
@@ -266,6 +302,16 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
             raise ValueError(f"cache_batch_idx[{i}] = {slot} is outside the {n_pages}-slot cache")
         if not 0 <= lp <= lens[i]:
             raise ValueError(f"cache_leftpad[{i}] = {lp} is outside [0, cache_seqlens[{i}]] = [0, {lens[i]}]")
+    # shared prefixes (prefix_k, prefix_v, prefix_seqlens, prefix_k_descale, prefix_v_descale): sequence i reads
+    # rows [0, plens[i // n]) of prefix i // n ahead of its own keys
+    plens = []
+    if prefix is not None:
+        pk, pv, pseq, pkd, pvd = prefix
+        n_per = b // pk.shape[0]
+        plens = pseq.tolist()
+        for j, x in enumerate(plens):
+            if not 0 <= x <= pk.shape[1]:
+                raise ValueError(f"prefix_seqlens[{j}] = {x} is outside [0, P_cap] = [0, {pk.shape[1]}]")
     if k is not None:  # rows past the capacity (or whose page is outside the pool) are dropped, as in the kernel path
         if fp8 and k.dtype != torch.float8_e4m3fn:  # pre-quantised e4m3 k / v are stored as they are
             k = torch.cat([quantize_e4m3(k[lo:lo + n], k_descale[i]) for i, (lo, n) in enumerate(spans)])
@@ -289,7 +335,8 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
         n_new = cnt if k is not None else 0
         n_keys = min(n + n_new, s_cap)
         lp = pads[i]  # rows [lp, n_keys) of the slot
-        if n_keys == lp or cnt == 0:
+        n_pre = plens[i // n_per] if prefix is not None else 0
+        if n_keys - lp + n_pre == 0 or cnt == 0:
             continue
         if table is None:
             kk, vv = k_cache[slots[i], lp:n_keys], v_cache[slots[i], lp:n_keys]
@@ -300,8 +347,15 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
             kk, vv = k_cache[pages].flatten(0, 1)[:n_keys], v_cache[pages].flatten(0, 1)[:n_keys]
         if fp8:  # the dequantised rows
             kk, vv = kk.float() * k_descale[i][:, None], vv.float() * v_descale[i][:, None]
-        # appended key u (row n + u) is visible to token t iff u <= t, i.e. row j <= t + n (j counted from lp)
-        diag = n - lp if (n_new and causal) else None
+        if n_pre:  # the prefix rows come first, and every query token sees them
+            p = i // n_per
+            pkk, pvv = pk[p, :n_pre], pv[p, :n_pre]
+            if fp8:
+                pkk, pvv = pkk.float() * pkd[p][:, None], pvv.float() * pvd[p][:, None]
+            kk, vv = torch.cat([pkk.to(kk.dtype), kk]), torch.cat([pvv.to(vv.dtype), vv])
+        # appended key u (row n + u) is visible to token t iff u <= t, i.e. row j <= t + n (j counted from lp, after
+        # the prefix rows)
+        diag = n_pre + n - lp if (n_new and causal) else None
         out[lo:lo + cnt], lse[:, lo:lo + cnt] = block_fwd(q[lo:lo + cnt], kk, vv, softmax_scale, diag)
     if world > 1:
         parts = _gather(torch.cat([out.reshape(-1), lse.reshape(-1)]), pg, world)
@@ -328,7 +382,10 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
               cu_seqlens_q: Optional[Tensor], max_seqlen_q: int, rotary_cos: Optional[Tensor] = None,
               rotary_sin: Optional[Tensor] = None, rotary_seqlens: Optional[Tensor] = None,
               rotary_interleaved: bool = True, q_descale: Optional[Tensor] = None,
-              cache_batch_idx: Optional[Tensor] = None, cache_leftpad: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+              cache_batch_idx: Optional[Tensor] = None, cache_leftpad: Optional[Tensor] = None,
+              prefix_k_cache: Optional[Tensor] = None, prefix_v_cache: Optional[Tensor] = None,
+              prefix_seqlens: Optional[Tensor] = None, prefix_k_descale: Optional[Tensor] = None,
+              prefix_v_descale: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
     """q (B, Sq, Hq, D) -> (out (B, Sq, Hq, D) in q.dtype (bf16 for an e4m3 q), lse (B, Hq, Sq) fp32).  ``k`` /
     ``v`` are appended to the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's
     name ("" = world); with ``block_table`` the caches are this rank's page pools; e4m3 caches come with contiguous
@@ -336,7 +393,9 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
     (total_q, Hq, D) and lse (Hq, total_q); ``max_seqlen_q`` bounds the counts (0 when uniform).  With
     ``rotary_cos`` / ``rotary_sin`` / ``rotary_seqlens``, every rank rotates q and the append rank rotates k before
     it stores it.  An e4m3 q comes with a contiguous fp32 (B, Hkv) ``q_descale``.  ``cache_batch_idx`` /
-    ``cache_leftpad`` (B,) int32 pick each sequence's cache slot and first key row."""
+    ``cache_leftpad`` (B,) int32 pick each sequence's cache slot and first key row.  ``prefix_k_cache`` /
+    ``prefix_v_cache`` (P, P_cap, Hkv, D) with ``prefix_seqlens`` (P,) int32 (and fp32 (P, Hkv) descales for e4m3)
+    are this rank's shards of the prefixes shared by consecutive groups of B / P sequences (read-only)."""
     pg = resolve_group(group)
     rank, world = group_info(pg)
     if k is not None and not 0 <= append_rank < world:
@@ -349,17 +408,23 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
                              cu_seqlens_q=cu_seqlens_q, max_seqlen_q=max_seqlen_q, rotary_cos=rotary_cos,
                              rotary_sin=rotary_sin, rotary_seqlens=rotary_seqlens,
                              rotary_interleaved=rotary_interleaved, q_descale=q_descale,
-                             cache_batch_idx=cache_batch_idx, cache_leftpad=cache_leftpad)
+                             cache_batch_idx=cache_batch_idx, cache_leftpad=cache_leftpad,
+                             prefix_k_cache=prefix_k_cache, prefix_v_cache=prefix_v_cache,
+                             prefix_seqlens=prefix_seqlens, prefix_k_descale=prefix_k_descale,
+                             prefix_v_descale=prefix_v_descale)
     rotary = None if rotary_cos is None else (rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved)
+    prefix = None if prefix_k_cache is None else (prefix_k_cache, prefix_v_cache, prefix_seqlens, prefix_k_descale,
+                                                  prefix_v_descale)
     return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table,
                          k_descale, v_descale, cu_seqlens_q, max_seqlen_q, rotary, q_descale, cache_batch_idx,
-                         cache_leftpad)
+                         cache_leftpad, prefix)
 
 
 @cp_decode.register_fake
 def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group, block_table, k_descale,
       v_descale, cu_seqlens_q, max_seqlen_q, rotary_cos=None, rotary_sin=None, rotary_seqlens=None,
-      rotary_interleaved=True, q_descale=None, cache_batch_idx=None, cache_leftpad=None):
+      rotary_interleaved=True, q_descale=None, cache_batch_idx=None, cache_leftpad=None, prefix_k_cache=None,
+      prefix_v_cache=None, prefix_seqlens=None, prefix_k_descale=None, prefix_v_descale=None):
     out = q.new_empty(q.shape, dtype=_out_dtype(q))
     if cu_seqlens_q is not None:
         total_q, hq, _ = q.shape
@@ -408,6 +473,52 @@ def _check_cache_index(name, x, q, b):
         raise ValueError(f"{name} must be on q's device")
 
 
+def _check_prefix(q, k_cache, pk, pv, pseq, pkd, pvd, b, hkv, d):
+    """Checks the shared prefixes and returns their descales as the contiguous (P, Hkv) fp32 tensors the kernels read
+    (None for bf16 / fp16 caches)."""
+    if pk is None or pv is None or pseq is None:
+        raise ValueError("pass prefix_k_cache, prefix_v_cache and prefix_seqlens together")
+    if q.dtype == torch.float8_e4m3fn:
+        raise ValueError("a shared prefix needs a bf16 / fp16 q: q_descale varies per sequence inside a packed prefix "
+                         "tile, which fp8 (e4m3) queries with a prefix do not support")
+    for name, x, c in (("prefix_k_cache", pk, k_cache), ("prefix_v_cache", pv, k_cache)):
+        if not isinstance(x, Tensor) or x.dim() != 4 or not x.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous (P, P_cap, Hkv, D) tensor")
+        if x.dtype != c.dtype:
+            raise ValueError(f"{name} must have the cache's dtype ({c.dtype}), not {x.dtype}")
+    if pk.shape != pv.shape or tuple(pk.shape[2:]) != (hkv, d):
+        raise ValueError(f"prefix_k_cache {tuple(pk.shape)} and prefix_v_cache {tuple(pv.shape)} must both be "
+                         f"(P, P_cap, Hkv, D) with (Hkv, D) = {(hkv, d)}")
+    n_prefix, p_cap = pk.shape[:2]
+    if n_prefix < 1 or p_cap < 1 or n_prefix * p_cap >= 2 ** 31:
+        raise ValueError(f"prefix caches: P = {n_prefix} and P_cap = {p_cap} must be >= 1 with P * P_cap < 2^31")
+    if pk.device != q.device or pv.device != q.device:
+        raise ValueError("prefix_k_cache / prefix_v_cache must be on q's device")
+    if b % n_prefix != 0:
+        raise ValueError(f"the batch (B = {b}) must be a multiple of the prefix count (P = {n_prefix}): sequence b "
+                         "uses prefix b // (B // P)")
+    if (not isinstance(pseq, Tensor) or pseq.dtype != torch.int32 or tuple(pseq.shape) != (n_prefix,)
+            or not pseq.is_contiguous()):
+        raise ValueError(f"prefix_seqlens must be a contiguous (P,) = ({n_prefix},) int32 tensor")
+    if pseq.device != q.device:
+        raise ValueError("prefix_seqlens must be on q's device")
+    if k_cache.dtype != torch.float8_e4m3fn:
+        if pkd is not None or pvd is not None:
+            raise ValueError("prefix_k_descale / prefix_v_descale are only taken with fp8 (float8_e4m3fn) caches")
+        return None, None
+    out = []
+    for name, x in (("prefix_k_descale", pkd), ("prefix_v_descale", pvd)):
+        if x is None:
+            raise ValueError(f"fp8 prefix caches need {name} (fp32, shape (), (Hkv,) or (P, Hkv))")
+        if not isinstance(x, Tensor) or x.dtype != torch.float32 or x.device != q.device:
+            raise ValueError(f"fp8 {name} must be a float32 tensor on q's device")
+        if tuple(x.shape) not in ((), (hkv,), (n_prefix, hkv)):
+            raise ValueError(f"fp8 {name} must have shape (), (Hkv,) or (P, Hkv) = {(n_prefix, hkv)}, not "
+                             f"{tuple(x.shape)}")
+        out.append(x.expand(n_prefix, hkv).contiguous())
+    return tuple(out)
+
+
 def _check_rotary(cos, sin, rotary_seqlens, q, b, d, cache_seqlens, group):
     """Checks the rotary tables and returns the (B,) positions the kernels read: ``rotary_seqlens``, or
     ``cache_seqlens`` in a one-rank group."""
@@ -446,7 +557,8 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
                                block_table=None, k_descale=None, v_descale=None, cu_seqlens_q=None,
                                max_seqlen_q=None, rotary_cos=None, rotary_sin=None, rotary_interleaved=True,
                                rotary_seqlens=None, window_size=(-1, -1), alibi_slopes=None, q_descale=None,
-                               cache_batch_idx=None, cache_leftpad=None):
+                               cache_batch_idx=None, cache_leftpad=None, prefix_k_cache=None, prefix_v_cache=None,
+                               prefix_seqlens=None, prefix_k_descale=None, prefix_v_descale=None):
     """Decode attention of new query tokens against a KV cache sharded over ``group`` (modelled on flash-attn's
     ``flash_attn_with_kvcache``).  Inference only: no gradient.
 
@@ -499,6 +611,27 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
       their current contents) and does not validate them: an index outside ``[0, B_cache)`` or a pad outside
       ``[0, cache_seqlens[b]]`` gives an undefined result but no access outside the caches (the sequence sees no key
       on this rank and its append is dropped; the pad is clamped).  The dense path raises ``ValueError`` for both.
+    * Shared prefixes (one long prompt, many continuations: best-of-n, parallel sampling, RL rollouts, one system
+      prompt under many requests): ``prefix_k_cache`` / ``prefix_v_cache`` ``(P, P_cap, Hkv, D)``, contiguous, in the
+      dtype of ``k_cache`` / ``v_cache``, are this rank's shard of ``P >= 1`` prompts, with ``B % P == 0`` and
+      ``P * P_cap < 2**31``.  Sequence ``b`` uses prefix ``b // (B // P)``: the ``B / P`` samples of a prompt are
+      consecutive (``repeat_interleave`` order).  ``prefix_seqlens`` ``(P,)`` int32 on q's device, contiguous, gives
+      the valid rows of each prefix shard on this rank (0 is allowed); each rank passes its own.  With e4m3 caches
+      ``prefix_k_descale`` / ``prefix_v_descale`` (fp32, ``()``, ``(Hkv,)`` or ``(P, Hkv)``) are required, as
+      ``k_descale`` is.  On this rank sequence ``b`` sees rows ``[0, prefix_seqlens[p])`` of its prefix, visible to
+      every query token with or without ``causal``, followed by everything it sees without a prefix: its own cache
+      (slots, left pad, pages, e4m3), and the appended tokens under the causal rule.  ``k`` / ``v`` go to the
+      sequence's own cache; the prefix is never written.  ``cache_seqlens`` still counts the sequence's own rows
+      (0 is allowed).  The result is that of a plain call on a cache holding the prefix rows followed by the
+      sequence's rows, up to fp32 summation order; rotary positions are those of that plain call, so in a one-rank
+      group ``rotary_seqlens`` defaults to ``prefix_seqlens[p] + cache_seqlens[b]``.  The kernel runs a second pass in
+      which the query rows of a prompt's samples share one 64-row tile and each prefix K / V tile is read once for all
+      of them; its partials merge with the suffix pass's in the one combine.  ``prefix_seqlens`` is read on the device
+      only and clamped to ``[0, P_cap]`` (a CUDA graph replay uses its current contents); the dense path raises
+      ``ValueError`` for a value outside that range.  Missing pieces, shape / dtype / device / contiguity mismatches,
+      ``B % P != 0`` and an e4m3 ``q`` with a prefix (``q_descale`` would vary inside a packed prefix tile) raise
+      ``ValueError``.  Paged prefixes, prefixes shared by non-consecutive sequences and nested prefixes are not
+      supported.
     * ``k`` / ``v`` ``(B, Sq, Hkv, D)``, optional, the same on every rank: written in place into the caches of rank
       ``append_rank`` only, at rows ``[cache_seqlens[b], cache_seqlens[b] + Sq)``, before attention (rows past
       ``S_cap`` are dropped).  The caller advances ``cache_seqlens``.  ``append_rank`` is required with ``k`` / ``v``
@@ -644,11 +777,21 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
                 raise ValueError(f"k / v must be (B, Sq, Hkv, D) = {(b, sq, hkv, d)} in q's dtype")
     elif append_rank is not None:
         raise ValueError("append_rank must be None when no k / v are given")
+    has_prefix = prefix_k_cache is not None or prefix_v_cache is not None or prefix_seqlens is not None
+    if has_prefix:
+        prefix_k_descale, prefix_v_descale = _check_prefix(q, k_cache, prefix_k_cache, prefix_v_cache, prefix_seqlens,
+                                                           prefix_k_descale, prefix_v_descale, b, hkv, d)
+    elif prefix_k_descale is not None or prefix_v_descale is not None:
+        raise ValueError("prefix_k_descale / prefix_v_descale are only taken with prefix_k_cache / prefix_v_cache")
     if rotary_cos is not None or rotary_sin is not None:
         if q8:
             raise ValueError("rotary_cos / rotary_sin need a bf16 / fp16 q: the rotation belongs before quantisation, "
                              "so rotate q and k, then quantise them")
+        default_pos = rotary_seqlens is None
         rotary_seqlens = _check_rotary(rotary_cos, rotary_sin, rotary_seqlens, q, b, d, cache_seqlens, group)
+        if default_pos and has_prefix:  # the keys before the new tokens: the prefix rows, then the sequence's own
+            rotary_seqlens = (cache_seqlens + prefix_seqlens.repeat_interleave(b // prefix_seqlens.shape[0])).to(
+                torch.int32)
         if k is None:
             raise ValueError("rotary_cos / rotary_sin need k / v: the rotation applies to the new tokens")
     elif rotary_seqlens is not None:
@@ -657,5 +800,6 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
     out, lse = cp_decode(q, k_cache, v_cache, cache_seqlens, k, v, -1 if append_rank is None else int(append_rank),
                          scale, bool(causal), group_name(group), block_table, k_descale, v_descale, cu_seqlens_q,
                          max_seqlen_q if varlen else 0, rotary_cos, rotary_sin, rotary_seqlens,
-                         bool(rotary_interleaved), q_descale, cache_batch_idx, cache_leftpad)
+                         bool(rotary_interleaved), q_descale, cache_batch_idx, cache_leftpad, prefix_k_cache,
+                         prefix_v_cache, prefix_seqlens, prefix_k_descale, prefix_v_descale)
     return (out, lse) if return_softmax_lse else out
