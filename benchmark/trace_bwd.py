@@ -21,9 +21,12 @@ from ring_flash_attn_b200.ops import cuda_ext  # noqa: E402
 NAMES = ["S^T ready", "dP^T ready", "dS^T staged", "dQ issued", "dQ complete", "dQ reduced", "S^T issued",
          "dV/dK issued"]
 # (label, (tile offset, slot) from, (tile offset, slot) to): intervals inside tile i or from tile i to tile i + 1
+# (the next tile's S^T is issued right after this tile's dQ GEMM, before the wait for dQ and the dQ staging)
 INTERVALS = [
-    ("dQ issued -> dQ complete", (0, 3), (0, 4)),
-    ("dQ complete -> next S^T issued", (0, 4), (1, 6)),
+    ("dQ issued -> next S^T issued", (0, 3), (1, 6)),
+    ("next S^T issued -> dQ complete", (1, 6), (0, 4)),
+    ("dQ complete -> dQ reduce-add issued", (0, 4), (0, 5)),
+    ("dQ reduce-add issued -> next S^T ready", (0, 5), (1, 0)),
     ("S^T issued -> S^T ready", (0, 6), (0, 0)),
     ("dP^T ready -> dV/dK issued", (0, 1), (0, 7)),
     ("cycles per tile (S^T ready -> next S^T ready)", (0, 0), (1, 0)),

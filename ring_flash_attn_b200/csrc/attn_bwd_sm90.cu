@@ -15,14 +15,18 @@
 //   dK_w += dS^T Q_i         (A = dS^T from registers, B = Q MN-major)
 //   dQ_i[:, 64 w : 64 w + 64] = dS_i K[:, 64 w : 64 w + 64]   (A = dS^T of both groups in shared memory,
 //                            read MN-major; B = K MN-major) -> fp32 shared memory (128-byte swizzled boxes of
-//                            32 dims) -> TMA reduce-add
-// Both warpgroups meet at three named barriers per query tile (dS^T complete, dQ staged, previous tile retired),
-// so the Q / dO ring needs no "empty" barriers: thread 0 refills the stage of tile i - 1 while tile i runs.
+//                            32 dims) -> TMA reduce-add of the group's own two boxes, issued by its thread 0
+// Both warpgroups meet at two named barriers per query tile (previous tile retired, dS^T complete), so the Q / dO
+// ring needs no "empty" barriers: thread 0 refills the stage of tile i - 1 while tile i runs.  At head dim 128,
+// between the dQ GEMM and the next tile's S^T each group only meets its own 128 threads, around its dQ staging (at
+// head dim 64 group 0 stages all of dQ and both groups meet there).  The loader's tile iterator lives in shared
+// memory.
 // Each stage also holds the 64 lse and delta values of its rows and a description of its tile.  Threads 0-63 copy
 // lse / delta for tile i + 2 (one row each, coalesced, cp.async: no register held in flight) at the top of tile i
 // and wait for the copies before its first barrier, so the softmax reads shared memory and no global load sits
 // between a GEMM's completion and the exp2 that needs it.  S^T and dP^T are separate commit groups: P^T is
-// computed while dP^T still runs.
+// computed while dP^T still runs.  S^T of tile i + 1 is issued right after the dQ GEMM of tile i, before the wait
+// for dQ, so the tensor pipe works on it while dQ of tile i is staged and its reduce-add issued.
 #include <math_constants.h>
 #include <stdio.h>
 
@@ -73,7 +77,6 @@ struct alignas(16) StageTile {
   int ti, diag, lo;
   int head, row;  // of the tile's dQ rows (first row)
 };
-static_assert(sizeof(Barriers) + kStages * sizeof(StageTile) <= 1024, "barrier area");
 
 // Query tiles of one segment that can see this key tile.
 struct QGeom {
@@ -129,6 +132,8 @@ struct TileIter {
     settle();
   }
 };
+
+static_assert(sizeof(Barriers) + kStages * sizeof(StageTile) + sizeof(TileIter) <= 1024, "barrier area");
 
 template <typename T, bool kWindow, int kD>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -188,32 +193,30 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   // ---------------------------------------------------------------- loads (threads 0-63; TMA: thread 0)
   // (a tile no local query reaches only sends zero rows: nothing is loaded, and in particular no TMA write can
   // land in the K | V area after the epilogue has started to stage those rows there)
-  TileIter ld;
-  ld.init(p.qsegs, it.seg_begin, it.seg_count, group);
-  int n_loaded = 0;
-  auto load_next = [&]() {
-    if (tid == 0) {
-      const int stage = n_loaded % kStages;
-      const int head = kv_head * group + ld.gq;
-      const int row = ld.g.q_row0 + ld.ti * kTileQ;
-      uint8_t* dq_ = smem_qdo + stage * 2 * kQBytes;
-      uint8_t* ddo = dq_ + kQBytes;
-      mbar_arrive_expect_tx(&bars->qdo_full[stage], 2 * kQBytes);
+  // The loader's iterator: threads 0-63 walk it in registers over the first kStages - 1 tiles; from then on it
+  // lives in shared memory and thread 0 advances it after each refill, so it holds no register across the loop.
+  TileIter* ld_smem = reinterpret_cast<TileIter*>(tiles + kStages);
+  // Q / dO of tile n (at `ld`) -> stage n % kStages; thread 0
+  auto load_tile = [&](const TileIter& ld, int n) {
+    const int stage = n % kStages;
+    const int head = kv_head * group + ld.gq;
+    const int row = ld.g.q_row0 + ld.ti * kTileQ;
+    uint8_t* dq_ = smem_qdo + stage * 2 * kQBytes;
+    uint8_t* ddo = dq_ + kQBytes;
+    mbar_arrive_expect_tx(&bars->qdo_full[stage], 2 * kQBytes);
 #pragma unroll
-      for (int h = 0; h < kSubTiles; ++h) {
-        tma_load_3d(dq_ + h * kQHalf, &tm_q, &bars->qdo_full[stage], 64 * h, head, row);
-        tma_load_3d(ddo + h * kQHalf, &tm_do, &bars->qdo_full[stage], 64 * h, head, row);
-      }
-      // (its slot was last read by tile n_loaded - kStages, which every thread finished before barrier 1)
-      tiles[stage] = StageTile{ld.ti, ld.g.diag, ld.g.lo, head, row};
+    for (int h = 0; h < kSubTiles; ++h) {
+      tma_load_3d(dq_ + h * kQHalf, &tm_q, &bars->qdo_full[stage], 64 * h, head, row);
+      tma_load_3d(ddo + h * kQHalf, &tm_do, &bars->qdo_full[stage], 64 * h, head, row);
     }
-    ++n_loaded;
-    ld.next();
+    // (its slot was last read by tile n - kStages: by every thread before barrier 1 of that tile, and by the
+    // threads that issue its dQ reduce-add before barrier 1 of the next tile, which precedes this refill)
+    tiles[stage] = StageTile{ld.ti, ld.g.diag, ld.g.lo, head, row};
   };
-  // lse and delta of row `tid` of the tile being loaded -> the stage's slots, with cp.async (no register is held
-  // while the copy is in flight; complete after cp_async_wait_all).  Rows that do not exist: lse -inf, delta 0.
-  auto lse_stage = [&]() {
-    const uint32_t sl = lse_base + ((n_loaded % kStages) * kTileQ + tid) * 4;
+  // lse and delta of row `tid` of tile n (at `ld`) -> the stage's slots, with cp.async (no register is held while
+  // the copy is in flight; complete after cp_async_wait_all).  Rows that do not exist: lse -inf, delta 0.
+  auto lse_stage = [&](const TileIter& ld, int n) {
+    const uint32_t sl = lse_base + ((n % kStages) * kTileQ + tid) * 4;
     const int qi = ld.ti * kTileQ + tid;
     if (qi < ld.g.q_len) {
       const int row = ld.g.q_row0 + qi;
@@ -254,10 +257,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     }
   }
   if (tid < kTileQ) {
-    while (n_loaded < kStages - 1 && n_loaded < total_tiles) {
-      lse_stage();
-      load_next();
+    TileIter ld;
+    ld.init(p.qsegs, it.seg_begin, it.seg_count, group);
+    for (int n = 0; n < kStages - 1 && n < total_tiles; ++n) {
+      lse_stage(ld, n);
+      if (tid == 0) load_tile(ld, n);
+      ld.next();
     }
+    if (tid == 0) *ld_smem = ld;
     cp_async_wait_all();
   }
   __syncthreads();
@@ -277,19 +284,17 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const uint64_t ds_mn = gmma_desc(smem_u32(smem_ds), kDSBytes);      // dS (64 queries x 128 keys), MN-major A
   const uint64_t k_mn = gmma_desc(k_base + w * kKVHalf, kKVHalf);     // K[:, 64 w : 64 w + 64], MN-major B
 
-  if (total_tiles > 0) mbar_wait(&bars->kv_full, 0);
-  for (int i = 0; i < total_tiles; ++i) {
-    const int stage = i % kStages;
-    const StageTile g = tiles[stage];
-    const int ti = g.ti;
-    // lse / delta of tile i + 2 into the slot of tile i - 1 (whose softmax every thread finished before the
-    // barriers of tile i - 1): copied under this tile's GEMMs and softmax, complete before barrier 1
-    if (tid < kTileQ && n_loaded < total_tiles) lse_stage();
-    mbar_wait(&bars->qdo_full[stage], (i / kStages) & 1);
-    const uint32_t st_off = stage * 2 * kQBytes;
-
-    // ---- S^T, dP^T (two commit groups)
-    float st[32], dpt[32];
+  const bool do_dq = kD == 128 || w == 0;  // head dim 64: group 0 computes all of dQ
+  float st[32];
+  // ---- top of tile n: lse / delta copies of tile n + 2, the stage wait, S^T issued (one commit group).  Called
+  // for n = total_tiles too (after the last tile): that S^T reads whatever stage n % kStages holds and is never
+  // used, but the issue stays unconditional (a conditional wgmma issue makes ptxas serialise every wgmma).
+  auto issue_st = [&](int n) {
+    // lse / delta of tile n + 2 go into the slot of tile n - 1, whose softmax every thread finished before the
+    // barriers of tile n - 1; they are copied under tile n's GEMMs and softmax and complete before its barrier 1
+    if (tid < kTileQ && n + kStages - 1 < total_tiles) lse_stage(*ld_smem, n + kStages - 1);
+    if (n < total_tiles) mbar_wait(&bars->qdo_full[n % kStages], (n / kStages) & 1);
+    const uint32_t st_off = (n % kStages) * 2 * kQBytes;
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < kD / 16; ++k) {
@@ -298,7 +303,21 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       Gmma<T>::template ss64<0, 0>(st, gmma_desc_add(k_km, oa), gmma_desc_add(q_km0, ob), k > 0);
     }
     wgmma_commit();
-    RFA_STAMP(tid == 0, i, 6);
+    RFA_STAMP(tid == 0, n, 6);
+  };
+  if (total_tiles > 0) {
+    mbar_wait(&bars->kv_full, 0);
+    issue_st(0);
+  }
+  for (int i = 0; i < total_tiles; ++i) {
+    const int stage = i % kStages;
+    const StageTile g = tiles[stage];
+    const int ti = g.ti;
+    const uint32_t st_off = stage * 2 * kQBytes;
+
+    // ---- dP^T (S^T of this tile was issued at the end of the previous one; two commit groups)
+    float dpt[32];
+    wgmma_fence();
 #pragma unroll
     for (int k = 0; k < kD / 16; ++k) {
       const uint32_t oa = (k >> 2) * kKVHalf + (k & 3) * 32;
@@ -378,12 +397,18 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     wgmma_commit();
     RFA_STAMP(tid == 0, i, 7);
 
-    // tile i - 1 has retired everywhere past this barrier: its dQ has been read out of smem_dq by the reduce, the
-    // dQ GEMMs no longer read smem_ds, and its Q / dO stage may be refilled
+    // tile i - 1 has retired everywhere past this barrier: the dQ GEMMs no longer read smem_ds, and its Q / dO
+    // stage may be refilled
     if (tid < kTileQ) cp_async_wait_all();
-    if (tid == 0) tma_store_wait_read<0>();
     named_bar_sync(1, kThreads);
-    if (tid < kTileQ && n_loaded < total_tiles) load_next();
+    // (thread 0 advances the loader's iterator; the other loader threads read it at the top of tile i + 1, after
+    // barrier 2)
+    if (tid == 0 && i + kStages - 1 < total_tiles) {
+      TileIter ld = *ld_smem;
+      load_tile(ld, i + kStages - 1);
+      ld.next();
+      *ld_smem = ld;
+    }
 
     // ---- dS^T -> shared memory: [128 keys][64 queries] bf16, 128-byte swizzled rows
 #pragma unroll
@@ -396,12 +421,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
             Pack2<T>::pack(dpt[4 * j + 2 * h], dpt[4 * j + 2 * h + 1]);
     }
     fence_proxy_async_smem();
+    // this group's dQ boxes of tile i - 1 have been read out by its reduce-add before the group stages tile i's
+    if (wtid == 0) tma_store_wait_read<0>();
     named_bar_sync(2, kThreads);
     RFA_STAMP(tid == 0, i, 2);
 
-    // ---- dQ[:, 64 w : 64 w + 64] = dS K[:, 64 w : 64 w + 64]   (head dim 64: group 0 computes all of dQ)
+    // ---- dQ[:, 64 w : 64 w + 64] = dS K[:, 64 w : 64 w + 64]
     float dq[32];
-    const bool do_dq = w < kD / 64;
     if (do_dq) {
       wgmma_fence();
 #pragma unroll
@@ -410,7 +436,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       wgmma_commit();
     }
     RFA_STAMP(tid == 0, i, 3);
-    wgmma_wait<0>();
+    // ---- S^T of tile i + 1, so that the tensor pipe has it queued behind dQ while this tile's dQ is staged
+    issue_st(i + 1);
+    // commit groups in flight: dV / dK (i), dQ (i, groups that compute dQ), S^T (i + 1).  Groups complete in
+    // order: this retires those of tile i and leaves S^T (i + 1) running.  Past barrier 1 of tile i + 1 no GEMM of
+    // tile i runs anywhere: smem_ds may be rewritten and the stage of tile i refilled.
+    wgmma_wait<1>();
     fence_regs(dv);
     fence_regs(dk);
     RFA_STAMP(tid == 0, i, 4);
@@ -418,7 +449,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       fence_regs(dq);
       // smem_dq holds the tile as kD / 32 boxes of [64 queries][32 dims] fp32, 128-byte rows with the TMA 128-byte
       // swizzle (16-byte unit u of row q at u ^ (q & 7)), so that the eight rows one store instruction writes fall
-      // into distinct banks: 2 shared-memory wavefronts per warp store instead of 8 with 512-byte unswizzled rows
+      // into distinct banks: 2 shared-memory wavefronts per warp store instead of 8 with 512-byte unswizzled rows.
+      // Warpgroup w owns boxes 2 w and 2 w + 1 (dims [64 w, 64 w + 64)) and adds them itself: its 128 threads
+      // meet at their own barrier and its thread 0 issues the two reduce-adds, so the groups do not wait for each
+      // other between the dQ GEMM and the next tile's S^T.
       const int q0 = 16 * (wtid >> 5) + (lane >> 2);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -431,19 +465,25 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
               make_float2(dq[4 * j + 2 * h], dq[4 * j + 2 * h + 1]);
         }
       }
+      fence_proxy_async_smem();
     }
-    fence_proxy_async_smem();
-    named_bar_sync(3, kThreads);
-    if (tid == 0) {
+    // head dim 64: group 0 computes all of dQ, and both groups still meet here (letting group 1 run ahead into the
+    // next tile made the head-dim-64 backward slower on an H100)
+    if constexpr (kD == 128) named_bar_sync(6 + w, 128);
+    else named_bar_sync(3, kThreads);
+    if (do_dq && wtid == 0) {
 #pragma unroll
-      for (int b = 0; b < kD / 32; ++b)
+      for (int b = 2 * w; b < 2 * w + 2; ++b)
         tma_reduce_add_3d(&tm_dq, reinterpret_cast<uint8_t*>(smem_dq) + b * (kTileQ * 128), 32 * b, tiles[stage].head,
                           tiles[stage].row);
       tma_store_commit();
     }
     RFA_STAMP(tid == 0, i, 5);
   }
-  if (tid == 0) tma_store_wait<0>();
+  // the unused S^T issued after the last tile has retired, and every reduce-add of this group has been read out
+  // and written, before the epilogue reuses shared memory
+  wgmma_wait<0>();
+  if (wtid == 0) tma_store_wait<0>();
 
   // ---------------------------------------------------------------- epilogue: dK / dV -> global
   const bool remote = p.dkv.world > 0;
