@@ -37,6 +37,13 @@ prompt copied into each sample's contiguous cache ahead of its suffix (a plain c
 whose block tables share the prompt's pages.  Each line reports the HBM bytes each arm must read (from shapes), the
 largest difference between the arms' outputs, and the card's name, power limit and maximum SM clock (read in one
 ``nvidia-smi`` query).  ``--kv-dtype e4m3`` runs the three arms over e4m3 caches with one descale per kv head.
+With ``--tree W1,W2,...`` the run times speculative-tree verification instead: a full draft tree in which every node
+at depth i has Wi children (plus the root; ``4,2,2,1`` has 45 nodes and 16 leaves), one per sequence, against caches
+of ``--cache`` tokens, in three arms alternating in one loop, each appending its tokens: the tree call (``tree_mask``,
+Sq = nodes), the causal chain call of the same shape (what the mask costs), and one causal call per root-to-leaf
+path (what a caller without ``tree_mask`` must do).  Each line reports the node and leaf counts, the K + V bytes each
+arm streams (every 64-row tile of a call streams its sequence's shard), the largest difference between a node's row
+in the tree call and the same node's row in a per-path call, and the card's name, power limit and maximum SM clock.
 
     python benchmark/bench_decode.py                      # B in {1, 8}, caches of 32K..512K tokens per rank
     python benchmark/bench_decode.py --page-size 16       # also the paged kernel, pages of 16 rows
@@ -48,6 +55,7 @@ largest difference between the arms' outputs, and the card's name, power limit a
     python benchmark/bench_decode.py --leftpad 1000       # also a left-padded call against the plain one
     torchrun --nproc-per-node 2 benchmark/bench_decode.py
     python benchmark/bench_decode.py --shared-prefix 32768 131072 --samples 4 16   # one prompt, n samples
+    python benchmark/bench_decode.py --tree 4,2,2,1       # a 45-node draft tree: tree vs chain vs per-path calls
     python benchmark/bench_decode.py --dry-run            # shapes and byte counts only (no GPU)
 """
 import argparse
@@ -97,8 +105,17 @@ def parse_args(argv=None):
     ap.add_argument("--samples", type=int, nargs="+", default=[4, 16], help="samples per prompt (--shared-prefix)")
     ap.add_argument("--prompts", type=int, nargs="+", default=[1], help="prompts P per call (--shared-prefix)")
     ap.add_argument("--suffix", type=int, default=256, help="each sample's own cached rows (--shared-prefix)")
+    ap.add_argument("--tree", type=str, default=None, metavar="W1,W2,...",
+                    help="time tree verification instead: a full tree with Wi children per node at depth i")
     ap.add_argument("--dry-run", action="store_true")
     args = ap.parse_args(argv)
+    if args.tree is not None:
+        try:
+            args.tree = [int(x) for x in args.tree.split(",")]
+        except ValueError:
+            ap.error("--tree takes comma-separated positive ints, e.g. 4,2,2,1")
+        if not args.tree or min(args.tree) < 1 or len(tree_parents(args.tree)) > dec.MAX_TREE_TOKENS:
+            ap.error(f"--tree needs positive widths and at most {dec.MAX_TREE_TOKENS} nodes")
     if args.shared_prefix is not None and (min(args.shared_prefix) < 1 or args.suffix < 1 or min(args.samples) < 1
                                            or min(args.prompts) < 1):
         ap.error("--shared-prefix, --samples, --prompts and --suffix must be positive")
@@ -275,6 +292,115 @@ def shared_prefix_main(args):
         torch.cuda.empty_cache()
 
 
+def tree_parents(widths):
+    """Parent array (breadth-first, root first) of the full tree with widths[i] children per node at depth i."""
+    parents, level = [-1], [0]
+    for w in widths:
+        nxt = []
+        for p in level:
+            for _ in range(w):
+                parents.append(p)
+                nxt.append(len(parents) - 1)
+        level = nxt
+    return parents
+
+
+def tree_paths(parents):
+    """Root-to-leaf node lists, one per leaf."""
+    leaves = sorted(set(range(len(parents))) - set(parents))
+    paths = []
+    for leaf in leaves:
+        path, j = [], leaf
+        while j >= 0:
+            path.append(j)
+            j = parents[j]
+        paths.append(path[::-1])
+    return paths
+
+
+def tree_shapes(args, sm_count):
+    """One dict per tree configuration: tree size, split counts and the K + V bytes each arm streams."""
+    parents = tree_parents(args.tree)
+    n, paths = len(parents), tree_paths(parents)
+    hkv, d, g = args.hkv, args.head_dim, args.hq // args.hkv
+    tiles = -(-n * g // dec.ROWS_PER_CTA)  # 64-row tiles of the tree / chain call
+    path_tiles = sum(-(-len(p) * g // dec.ROWS_PER_CTA) for p in paths)
+    for b in args.batch:
+        for s in args.cache:
+            shard = s * hkv * d * 2 * 2  # one sequence's K + V after the append
+            yield dict(tree=",".join(map(str, args.tree)), tree_nodes=n, tree_leaves=len(paths),
+                       max_depth=len(args.tree), per_path_calls=len(paths), batch=b, cache_tokens=s, hq=args.hq,
+                       hkv=hkv, head_dim=d, row_tiles=tiles, tree_splits=dec.num_splits(b, n, args.hq, hkv, s, sm_count),
+                       tree_bytes=b * tiles * shard, chain_bytes=b * tiles * shard, per_path_bytes=b * path_tiles * shard)
+
+
+def tree_main(args):
+    """The three tree-verification arms, alternating in one loop (see the module docstring)."""
+    if args.dry_run:
+        for cfg in tree_shapes(args, args.sm_count):
+            print(json.dumps(cfg))
+        return
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_decode.py needs a CUDA device (use --dry-run without one)")
+    dev = torch.device("cuda", torch.cuda.current_device())
+    name, power, clock = card_settings()
+    sm = torch.cuda.get_device_properties(dev).multi_processor_count
+    hq, hkv, d = args.hq, args.hkv, args.head_dim
+    parents = tree_parents(args.tree)
+    n, paths = len(parents), tree_paths(parents)
+    anc = torch.zeros(n, n, dtype=torch.bool)
+    for i in range(n):
+        j = i
+        while j >= 0:
+            anc[i, j] = True
+            j = parents[j]
+    for cfg in tree_shapes(args, sm):
+        b, s = cfg["batch"], cfg["cache_tokens"]
+        torch.manual_seed(0)
+        q = torch.randn(b, n, hq, d, device=dev, dtype=torch.bfloat16)
+        k_new, v_new = (torch.randn(b, n, hkv, d, device=dev, dtype=torch.bfloat16) for _ in range(2))
+        kc, vc = (torch.randn(b, s, hkv, d, device=dev, dtype=torch.bfloat16) for _ in range(2))
+        sl = torch.full((b,), s - n, dtype=torch.int32, device=dev)  # the shard holds s rows after the append
+        mask = anc.to(dev).expand(b, n, n).contiguous()
+        scale = d ** -0.5
+        idx = [torch.tensor(p, device=dev) for p in paths]
+        pq = [q[:, i].contiguous() for i in idx]
+        pk = [k_new[:, i].contiguous() for i in idx]
+        pv = [v_new[:, i].contiguous() for i in idx]
+
+        def tree_call():
+            return dec.kernel_decode(q, kc, vc, sl, k_new, v_new, True, scale, tree_mask=mask)
+
+        def chain_call():
+            return dec.kernel_decode(q, kc, vc, sl, k_new, v_new, True, scale)
+
+        def per_path_call():
+            return [dec.kernel_decode(a, kc, vc, sl, x, y, True, scale)[0] for a, x, y in zip(pq, pk, pv)]
+
+        arms = {"tree": tree_call, "chain": chain_call, "per_path": per_path_call}
+        times = {k: [] for k in arms}
+        order = list(arms)
+        for r in range(6):  # alternate them in one run, each arm first in two of the rounds
+            for k in order[r % 3:] + order[:r % 3]:
+                times[k].append(time_us(arms[k], args.iters, args.warmup))
+        res = dict(cfg, card=name, power_limit=power, max_sm_clock=clock)
+        for k, ts in times.items():
+            us = min(ts)
+            res[f"{k}_us"] = round(us, 2)
+            res[f"{k}_us_all"] = [round(t, 2) for t in ts]
+            res[f"{k}_GBps"] = round(cfg[f"{k}_bytes"] / (us * 1e-6) / 1e9, 1)
+        res["tree_speedup_vs_per_path"] = round(res["per_path_us"] / res["tree_us"], 3)
+        res["tree_vs_chain"] = round(res["tree_us"] / res["chain_us"], 3)
+        tree_out = tree_call()[0].float()
+        diff = 0.0
+        for i, out in zip(idx, per_path_call()):  # node path[t]'s row in its per-path call
+            diff = max(diff, (tree_out[:, i] - out.float()).abs().max().item())
+        res["max_abs_diff_tree_vs_per_path"] = diff
+        print(json.dumps(res), flush=True)
+        del q, k_new, v_new, kc, vc, pq, pk, pv
+        torch.cuda.empty_cache()
+
+
 def card():
     name = torch.cuda.get_device_name(0)
     try:
@@ -300,6 +426,9 @@ def time_us(fn, iters, warmup):
 
 def main():
     args = parse_args()
+    if args.tree is not None:
+        tree_main(args)
+        return
     if args.shared_prefix is not None:
         shared_prefix_main(args)
         return

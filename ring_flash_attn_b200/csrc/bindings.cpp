@@ -397,6 +397,21 @@ at::Tensor lse_unflatten(const at::Tensor& lse, const at::Tensor& cu, int64_t ma
   return out;
 }
 
+// A tree mask of decode_fwd / decode_prefix_fwd: bool or uint8 (rows, sq) contiguous on q's device, with causal.
+const uint8_t* tree_mask_ptr(const c10::optional<at::Tensor>& tree_mask, const at::Tensor& q, int64_t rows,
+                             int64_t sq, bool causal, const char* what) {
+  if (!tree_mask.has_value()) return nullptr;
+  const at::Tensor& m = *tree_mask;
+  TORCH_CHECK(m.scalar_type() == at::kBool || m.scalar_type() == at::kByte, what,
+              ": tree_mask must be bool or uint8");
+  TORCH_CHECK(m.device() == q.device() && m.is_contiguous() && m.dim() == 2 && m.size(0) == rows && m.size(1) == sq,
+              what, ": tree_mask must be contiguous (B * Sq, Sq), or (total_q, max_seqlen_q) when varlen, on q's "
+              "device");
+  TORCH_CHECK(causal, what, ": a tree mask replaces the causal rule among the appended keys: it needs causal");
+  TORCH_CHECK(sq <= 128, what, ": a tree mask takes at most 128 new tokens per sequence (two key tiles)");
+  return static_cast<const uint8_t*>(m.data_ptr());
+}
+
 // Split-KV decode (csrc/decode_sm90.cu).  q (B, Sq, Hq, D); k_cache / v_cache (B, S_cap, Hkv, D) with mergeable
 // batch and sequence dimensions; seqlens (B,) int32; k_new / v_new (B, Sq, Hkv, D) contiguous, appended to the caches
 // before attention when given.  part: fp32 (n_splits, B*Sq*Hq*D + B*Hq*Sq), see DecodeParams.  With block_table
@@ -411,7 +426,9 @@ at::Tensor lse_unflatten(const at::Tensor& lse, const at::Tensor& cu, int64_t ma
 // k_new / v_new may be float8_e4m3fn over e4m3 caches (stored as they are), or bf16 / fp16 with an e4m3 q.
 // cache_batch_idx (B,) int32 (contiguous caches only): sequence b reads and appends slot cache_batch_idx[b] of
 // (B_cache, S_cap, Hkv, D) caches; cache_leftpad (B,) int32: its keys start at that row.  Both are read on the device
-// only (see DecodeParams).
+// only (see DecodeParams).  tree_mask (B * Sq, Sq), or (total_q, max_seqlen_q) when varlen, bool / uint8, with
+// causal: which appended keys each new token sees, and the rotary positions (see DecodeParams); read on the device
+// only.
 void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
                 const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
                 double scale, at::Tensor& part, const c10::optional<at::Tensor>& block_table,
@@ -420,7 +437,7 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
                 const c10::optional<at::Tensor>& rotary_cos, const c10::optional<at::Tensor>& rotary_sin,
                 const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved,
                 const c10::optional<at::Tensor>& q_descale, const c10::optional<at::Tensor>& cache_batch_idx,
-                const c10::optional<at::Tensor>& cache_leftpad) {
+                const c10::optional<at::Tensor>& cache_leftpad, const c10::optional<at::Tensor>& tree_mask) {
   const c10::cuda::CUDAGuard guard(q_in.device());
   const bool varlen = cu_seqlens_q.has_value();
   TORCH_CHECK(q_in.dim() == (varlen ? 3 : 4), "decode_fwd: q must be (B, Sq, Hq, D), or (total_q, Hq, D) with "
@@ -584,6 +601,7 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
     p.cache_batch = static_cast<int>(k_cache.size(0));
   }
   if (cache_leftpad.has_value()) p.cache_leftpad = cache_leftpad->data_ptr<int>();
+  p.tree_mask = tree_mask_ptr(tree_mask, q, rows, sq, causal, "decode_fwd");
   const TensorView kv{k_cache.data_ptr(), cache_rows, static_cast<int>(hkv), k_cache.stride(1), k_cache.stride(2)};
   const TensorView vv{v_cache.data_ptr(), cache_rows, static_cast<int>(hkv), v_cache.stride(1), v_cache.stride(2)};
   check(rfa::decode_fwd_launch(q8 ? rfa::kDtypeE4M3 : dtype_code(q), fp8 ? rfa::kDtypeE4M3 : dtype_code(q), kv, vv,
@@ -596,13 +614,14 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
 // mergeable first two dimensions, in q's dtype or both e4m3 with k_descale / v_descale fp32 (P, Hkv) contiguous.
 // Sequence b reads prefix b / (B / P), rows [0, prefix_seqlens[p]) (read on the device only, clamped to [0, P_cap]),
 // all visible to every query token.  part: the partial slabs of this pass, in decode_fwd's layout.  causal and the
-// rotary tensors position q's rotation as in decode_fwd.
+// rotary tensors position q's rotation as in decode_fwd, and so does tree_mask (which masks no prefix key).
 void decode_prefix_fwd(const at::Tensor& q_in, const at::Tensor& prefix_k, const at::Tensor& prefix_v,
                        const at::Tensor& prefix_seqlens, bool causal, double scale, at::Tensor& part,
                        const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale,
                        const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q,
                        const c10::optional<at::Tensor>& rotary_cos, const c10::optional<at::Tensor>& rotary_sin,
-                       const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved) {
+                       const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved,
+                       const c10::optional<at::Tensor>& tree_mask) {
   const c10::cuda::CUDAGuard guard(q_in.device());
   const bool varlen = cu_seqlens_q.has_value();
   TORCH_CHECK(q_in.dim() == (varlen ? 3 : 4), "decode_prefix_fwd: q must be (B, Sq, Hq, D), or (total_q, Hq, D) "
@@ -701,6 +720,7 @@ void decode_prefix_fwd(const at::Tensor& q_in, const at::Tensor& prefix_k, const
     p.seqlen_ro = static_cast<int>(rc.size(0));
     p.rotary_interleaved = rotary_interleaved ? 1 : 0;
   }
+  p.tree_mask = tree_mask_ptr(tree_mask, q, rows, sq, causal, "decode_prefix_fwd");
   const int64_t cache_rows = n_prefix * p_cap;
   const TensorView kv{prefix_k.data_ptr(), cache_rows, static_cast<int>(hkv), prefix_k.stride(1), prefix_k.stride(2)};
   const TensorView vv{prefix_v.data_ptr(), cache_rows, static_cast<int>(hkv), prefix_v.stride(1), prefix_v.stride(2)};
@@ -774,6 +794,20 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("lse_flatten", &lse_flatten);
   m.def("lse_unflatten", &lse_unflatten);
   m.def("decode_fwd", &decode_fwd);
+  // the same without tree_mask
+  m.def("decode_fwd", [](const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
+                         const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
+                         double scale, at::Tensor& part, const c10::optional<at::Tensor>& block_table,
+                         const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale,
+                         const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q,
+                         const c10::optional<at::Tensor>& rotary_cos, const c10::optional<at::Tensor>& rotary_sin,
+                         const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved,
+                         const c10::optional<at::Tensor>& q_descale, const c10::optional<at::Tensor>& cache_batch_idx,
+                         const c10::optional<at::Tensor>& cache_leftpad) {
+    decode_fwd(q, k_cache, v_cache, seqlens, k_new, v_new, causal, scale, part, block_table, k_descale, v_descale,
+               cu_seqlens_q, max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, q_descale,
+               cache_batch_idx, cache_leftpad, c10::nullopt);
+  });
   // the same without cache_batch_idx / cache_leftpad
   m.def("decode_fwd", [](const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
                          const c10::optional<at::Tensor>& k_new, const c10::optional<at::Tensor>& v_new, bool causal,
@@ -785,7 +819,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                          const c10::optional<at::Tensor>& q_descale) {
     decode_fwd(q, k_cache, v_cache, seqlens, k_new, v_new, causal, scale, part, block_table, k_descale, v_descale,
                cu_seqlens_q, max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, q_descale,
-               c10::nullopt, c10::nullopt);
+               c10::nullopt, c10::nullopt, c10::nullopt);
   });
   // the same without q_descale (a bf16 / fp16 q)
   m.def("decode_fwd", [](const at::Tensor& q, at::Tensor& k_cache, at::Tensor& v_cache, const at::Tensor& seqlens,
@@ -797,9 +831,20 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                          const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved) {
     decode_fwd(q, k_cache, v_cache, seqlens, k_new, v_new, causal, scale, part, block_table, k_descale, v_descale,
                cu_seqlens_q, max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, c10::nullopt,
-               c10::nullopt, c10::nullopt);
+               c10::nullopt, c10::nullopt, c10::nullopt);
   });
   m.def("decode_prefix_fwd", &decode_prefix_fwd);
+  // the same without tree_mask
+  m.def("decode_prefix_fwd", [](const at::Tensor& q, const at::Tensor& prefix_k, const at::Tensor& prefix_v,
+                                const at::Tensor& prefix_seqlens, bool causal, double scale, at::Tensor& part,
+                                const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale,
+                                const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q,
+                                const c10::optional<at::Tensor>& rotary_cos,
+                                const c10::optional<at::Tensor>& rotary_sin,
+                                const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved) {
+    decode_prefix_fwd(q, prefix_k, prefix_v, prefix_seqlens, causal, scale, part, k_descale, v_descale, cu_seqlens_q,
+                      max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, c10::nullopt);
+  });
   m.def("decode_combine", &decode_combine);
   rfa::bind_peer_mem(m);
 }

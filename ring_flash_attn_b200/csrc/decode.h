@@ -40,7 +40,8 @@ struct DecodeParams {
   const float* v_descale;
   // Rotary embeddings of the new tokens; rotary_cos == nullptr: none.  Columns [0, 2 * rotary_half) of q and of the
   // appended k are rotated (pairs (i, i + rotary_half), or (2i, 2i + 1) when interleaved) at position
-  // rotary_seqlens[b] + t for key t, and for query token t the same when causal, rotary_seqlens[b] otherwise.
+  // rotary_seqlens[b] + t for key t, and for query token t the same when causal, rotary_seqlens[b] otherwise (with a
+  // tree mask: see tree_mask).
   // Positions are clamped to [0, seqlen_ro - 1], so a bad rotary_seqlens never reads outside the tables.
   const void* rotary_cos;    // (seqlen_ro, rotary_half) contiguous, in q's dtype
   const void* rotary_sin;
@@ -60,6 +61,13 @@ struct DecodeParams {
   // Shared prefixes (decode_prefix_launch only): sequences [i * prefix_n, (i + 1) * prefix_n) share prefix i, whose
   // valid rows are seqlens[i] (clamped to [0, s_cap]) of a (P, s_cap, Hkv, D) cache; the descales are (P, Hkv).
   int prefix_n;
+  // Tree attention (speculative decoding), with causal set; nullptr: none.  Byte u of row cu[b] + t (b * sq + t
+  // uniform; row stride sq) is nonzero iff new token t of sequence b sees appended key u of its own call (u < n_b;
+  // later columns are ignored).  It replaces the causal rule among the appended keys only: every cached key stays
+  // visible.  New token t (query and key) is rotated at rotary_seqlens[b] + max(n_t - 1, 0), n_t = the nonzero
+  // bytes of its row (a tree node's depth).  sq <= 128, so the appended keys span at most two key tiles.  Read on the
+  // device only, never validated.
+  const uint8_t* tree_mask;  // (total_q, sq)
 };
 
 // Appends k_new / v_new (B, Sq, Hkv, D), contiguous, in q's dtype, at rows [seqlens[b], seqlens[b] + Sq) of the
@@ -80,7 +88,8 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
 // (the same layout as decode_fwd_launch's; a caller merges both passes' slabs with one decode_combine_launch).  The
 // caches k_prefix / v_prefix are (n_prefix, p.s_cap, Hkv, D) with mergeable first two dimensions; p.seqlens are the
 // prefixes' valid rows, p.k_descale / p.v_descale (n_prefix, Hkv) with e4m3 caches, p.prefix_n = B / n_prefix.
-// Every prefix key is visible to every query token (p.n_new must be 0); q is rotated as in decode_fwd_launch.  No
+// Every prefix key is visible to every query token (p.n_new must be 0); q is rotated as in decode_fwd_launch (with
+// p.tree_mask, at the depth positions; the mask does not mask prefix keys).  No
 // append, block table, cache slots, left pads or e4m3 q.  The grid is (n_splits, decode_prefix_slots(p), n_prefix *
 // Hkv): a CTA takes 64 consecutive packed rows of one group, rows [b0 * sq, (b0 + n) * sq) of a uniform q or
 // [cu[b0], cu[b0 + n]) of a varlen one (b0 = prefix * n), each row (sequence, token, head-in-group) in that order.

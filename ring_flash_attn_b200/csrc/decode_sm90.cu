@@ -41,6 +41,14 @@
 // columns are masked to -inf and their V rows are zeroed in shared memory before P V (the cache may hold anything
 // there, NaN included).
 //
+// Tree masks (kTree, launched when tree_mask is set; causal): n_vis(t) is the sequence's token count for every row, so
+// kmax, the split ranges and the V-row zeroing are those of a non-causal call, and the tiles holding appended keys
+// (key0 + kTile > seqlen, at most two per sequence) then set S = -inf where the row's mask byte for key
+// u = key0 + c - seqlen is 0.  Rotary positions of new tokens come from one helper (new_token_pos), the mask row's
+// depth with a mask.  The prefix pass masks nothing (its keys are visible to every row); its kTree instantiation,
+// launched with a mask and rotary, differs only in the rotary positions.  Without a mask the kernels are the ones
+// compiled before tree masks existed.
+//
 // Cache slots and left padding (contiguous caches): sequence b's keys live in slot cache_batch_idx[b] and start at
 // row lp = cache_leftpad[b].  Each CTA resolves both once and then runs on keys relative to lp: seqlens[b] - lp valid
 // rows under a capacity of S_cap - lp, so the key loop, masks and split ranges are those of a plain call on the
@@ -55,6 +63,7 @@
 // Everything runs as a call with cache slot i, seqlens[i] valid rows, no append (every prefix key is visible to every
 // row) and descales [i, kv head]; only the rotary position and the lse address need a row's own sequence and token.
 // Its partials go to slabs after the suffix pass's, and the one combine merges both.
+#include <limits.h>
 #include <math_constants.h>
 
 #include <type_traits>
@@ -78,13 +87,18 @@ constexpr int kThreads = 160;  // one compute warpgroup + one producer warp
 constexpr int kThreadsFp8 = 288;  // + one converter warpgroup
 constexpr int kKHalfBytes = kTile * 128;  // one 64-element-wide (128-byte) swizzled K / V sub-tile
 constexpr int kQHalfBytes = kRows * 128;  // the same for the query tile
+constexpr int kBarBytes = 1024;           // the ring's mbarriers
+// Tree masks: one 32-bit word per (tile w, row half h, compute thread), the thread's hidden columns of the two key
+// tiles that can hold appended keys, so the key loop reads one word instead of 32 mask bytes per row
+constexpr int kTreeHideBytes = 2 * 2 * 128 * 4;
 
-template <int kD, bool kFp8, bool kQ8>
+template <int kD, bool kFp8, bool kQ8, bool kTree = false>
 constexpr int smem_bytes() {
+  constexpr int tree = kTree ? kTreeHideBytes : 0;
   if constexpr (kQ8)
-    return kRows * kD + kF8StagesQ8 * kTile * kD + kVStagesQ8 * kTile * kD * 2 + 1024 /*barriers*/ +
+    return kRows * kD + kF8StagesQ8 * kTile * kD + kVStagesQ8 * kTile * kD * 2 + kBarBytes + tree +
            1024 /*align slack*/;
-  return kRows * kD * 2 + (kFp8 ? kStagesFp8 * kTile * kD * 3 : kStages * kTile * kD * 2) + 1024 /*barriers*/ +
+  return kRows * kD * 2 + (kFp8 ? kStagesFp8 * kTile * kD * 3 : kStages * kTile * kD * 2) + kBarBytes + tree +
          1024 /*align slack*/;
 }
 
@@ -109,9 +123,11 @@ struct LoadRing {
 };
 
 // Keys of the shard visible to token t of a sequence with n_q new tokens (see the file comment), at most cap, all
-// counted from the sequence's first key row.
+// counted from the sequence's first key row.  With a tree mask (kTree) every row gets all n_q appended keys here, and
+// the mask step of the key loop hides the ones its row may not see.
+template <bool kTree>
 __device__ __forceinline__ int key_limit(const DecodeParams& p, int seqlen, int cap, int n_q, int t) {
-  const int n_vis = p.n_new == 0 ? 0 : (p.causal ? t + 1 : n_q);
+  const int n_vis = p.n_new == 0 ? 0 : (p.causal && !kTree ? t + 1 : n_q);
   const int lim = seqlen + n_vis;
   return lim < cap ? lim : cap;
 }
@@ -132,6 +148,19 @@ __device__ __forceinline__ int2 q_rows(const DecodeParams& p, int b) {
 __device__ __forceinline__ int rotary_pos(const DecodeParams& p, int b, int t) {
   const long long x = static_cast<long long>(__ldg(p.rotary_seqlens + b)) + t;
   return x < 0 ? 0 : (x >= p.seqlen_ro ? p.seqlen_ro - 1 : static_cast<int>(x));
+}
+
+// Offset from rotary_seqlens[b] of new token t of sequence b: with a tree mask, its depth (the nonzero bytes among
+// the first n_b of its mask row, minus one; 0 for an empty row), for its query and its key alike; otherwise t for a
+// key or a causal query token, and 0 for a query token of a non-causal call.  kMaybeTree = false: no mask.
+template <bool kMaybeTree>
+__device__ __forceinline__ int new_token_pos(const DecodeParams& p, int b, int t, bool key) {
+  if (!kMaybeTree || p.tree_mask == nullptr) return key || p.causal ? t : 0;
+  const int2 r = q_rows(p, b);
+  const uint8_t* row = p.tree_mask + static_cast<long long>(r.x + t) * p.sq;
+  int n = 0;
+  for (int u = 0; u < r.y; ++u) n += __ldg(row + u) != 0;
+  return n > 0 ? n - 1 : 0;
 }
 
 template <typename T>
@@ -350,8 +379,9 @@ __device__ __forceinline__ uint64_t f8_desc(const uint8_t* tile) {
   return kD == 128 ? gmma_desc(smem_u32(tile), 0) : gmma_desc_sw64(smem_u32(tile));
 }
 
-// kQ8: e4m3 queries (T = bf16, kFp8 set); kPrefix: the shared-prefix pass.  See the file comment.
-template <typename T, int kD, bool kFp8, bool kQ8, bool kPrefix = false>
+// kQ8: e4m3 queries (T = bf16, kFp8 set); kPrefix: the shared-prefix pass; kTree: p.tree_mask is set.  See the file
+// comment.
+template <typename T, int kD, bool kFp8, bool kQ8, bool kPrefix = false, bool kTree = false>
 __global__ void __launch_bounds__(kFp8 ? kThreadsFp8 : kThreads, 1)
 decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
               const __grid_constant__ DecodeParams p) {
@@ -400,7 +430,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   seqlen -= lp;
   cap -= lp;
   // the last row of the tile sees the most keys (the limit never decreases with t)
-  const int kmax = key_limit(p, seqlen, cap, qr.y, (row0 + rows_here - 1) / group);
+  const int kmax = key_limit<kTree>(p, seqlen, cap, qr.y, (row0 + rows_here - 1) / group);
   const int j0 = split * p.tiles_per_split;
   int j1 = (kmax + kTile - 1) / kTile;
   if (j1 > j0 + p.tiles_per_split) j1 = j0 + p.tiles_per_split;
@@ -412,6 +442,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   uint8_t* smem_kv = smem + kQBytes;
   uint8_t* smem_f8 = smem_kv + kSlots * kSlotBytes;  // e4m3 caches only
   auto* bars = reinterpret_cast<Barriers<kQ8>*>(smem_f8 + (kFp8 ? L::kSlots * L::kSlotBytes : 0));
+  static_assert(sizeof(Barriers<kQ8>) <= kBarBytes, "the barriers outgrew their space");
   // the ring TMA fills
   uint8_t* smem_load = kFp8 ? smem_f8 : smem_kv;
   uint64_t* load_full = kFp8 ? bars->f8_full : bars->kv_full;
@@ -523,7 +554,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   const T* q = reinterpret_cast<const T*>(p.q);
 
   // Q tile: packed rows in the 128-byte swizzled K-major layout TMA would write; rows past the group are zero.  With
-  // rotary, chunks below rotary_dim are rotated on the way (token t's position; the first token's when not causal).
+  // rotary, chunks below rotary_dim are rotated on the way (at new_token_pos).
   if constexpr (kQ8) {
     // e4m3 Q tile: kD-byte rows in the swizzle TMA writes for the e4m3 K tile (no rotary: the caller quantised q)
     const uint8_t* q8 = static_cast<const uint8_t*>(p.q);
@@ -555,7 +586,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
         if (p.rotary_cos != nullptr && c < p.rotary_half / 4) {
           int rb = b, rt = t;  // the row's own sequence and token
           if constexpr (kPrefix) prefix_token(p, b * p.prefix_n, qr.x + t, rb, rt);
-          val = rotate_chunk<T>(val, q_row, c, rotary_pos(p, rb, p.causal ? rt : 0), p);
+          val = rotate_chunk<T>(val, q_row, c, rotary_pos(p, rb, new_token_pos<kTree>(p, rb, rt, false)), p);
         }
       }
       *reinterpret_cast<uint4*>(smem_q + (c >> 3) * kQHalfBytes + r * 128 + (((c & 7) ^ (r & 7)) << 4)) = val;
@@ -564,11 +595,45 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   fence_proxy_async_smem();
   named_bar_sync(1, 128);
 
+  // Tree mask: the tiles holding appended keys start at key tile0 (seqlen < tile0 + kTile) and, for a sequence with
+  // more than tile0 + kTile - seqlen new tokens, at tile0 + kTile (n_q <= kTile).  Bit 2 j + e of word (w, h) hides
+  // this thread's column 8 j + quad_col + e of row r_base + 8 h in tile w.  Each thread reads back only its own words.
+  // tile0 stays INT_MAX in splits that end before it: the key loop keeps one register for all of this, and only the
+  // CTAs that reach the appended keys read the mask.
+  [[maybe_unused]] int tile0 = INT_MAX;
+  [[maybe_unused]] uint32_t* tree_hide = nullptr;  // after the barriers (smem_bytes<..., kTree>)
+  if constexpr (kTree && !kPrefix) {
+    tree_hide = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(bars) + kBarBytes);
+    if (p.n_new > 0 && (j0 + n_tiles) * kTile > seqlen) {
+      tile0 = seqlen / kTile * kTile;
+#pragma unroll 1
+      for (int wh = 0; wh < 4; ++wh) {
+        const int r = r_base + 8 * (wh & 1);
+        uint32_t hide = 0u;
+        if (r < rows_here) {  // then qr.y >= 1
+          const uint8_t* mrow = p.tree_mask + static_cast<long long>(qr.x + (row0 + r) / group) * p.sq;
+          const int u0 = tile0 + (wh >> 1) * kTile + quad_col - seqlen;  // appended key of column quad_col
+          // every load is issued, at a column clamped into the row, so that the 32 are in flight together (a load
+          // under a branch would wait for the one before it)
+          uint8_t m[32];
+#pragma unroll
+          for (int i = 0; i < 32; ++i) m[i] = __ldg(mrow + clamp_to(u0 + 8 * (i >> 1) + (i & 1), 0, qr.y - 1));
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const int u = u0 + 8 * (i >> 1) + (i & 1);
+            if (u >= 0 && u < qr.y && m[i] == 0) hide |= 1u << i;
+          }
+        }
+        tree_hide[wh * 128 + tid] = hide;
+      }
+    }
+  }
+
   int lim[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int r = r_base + 8 * h;
-    lim[h] = r < rows_here ? key_limit(p, seqlen, cap, qr.y, (row0 + r) / group) : 0;
+    lim[h] = r < rows_here ? key_limit<kTree>(p, seqlen, cap, qr.y, (row0 + r) / group) : 0;
   }
   float o[kD / 2];
 #pragma unroll
@@ -657,6 +722,20 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             if (8 * j + quad_col + e >= c_lim) s[4 * j + 2 * h + e] = -CUDART_INF_F;
+          }
+        }
+      }
+    }
+    // ---- tree mask: appended key u = key0 + c - seqlen stays visible only where the row's mask byte is set
+    if constexpr (kTree) {
+      if (key0 >= tile0) {
+        const uint32_t* hide = tree_hide + (key0 - tile0) / kTile * 256 + tid;  // words (w, 0), (w, 1)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t bits = hide[128 * h];
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            if (bits >> i & 1u) s[4 * (i >> 1) + 2 * h + (i & 1)] = -CUDART_INF_F;
           }
         }
       }
@@ -784,7 +863,8 @@ __device__ __forceinline__ long long new_row(const DecodeParams& p, int b, int t
 
 // One block per (b, t) row of the new keys, blockIdx.y selects K or V.  16-byte chunks; rows past the capacity
 // are dropped, and so are rows whose page id lies outside the pool.  With rotary, the K chunks below rotary_dim are
-// rotated as elements of T (at position rotary_seqlens[b] + t) before they are stored; everything else is a byte copy.
+// rotated as elements of T (at rotary_seqlens[b] + new_token_pos) before they are stored; everything else is a byte
+// copy.
 template <typename T>
 __global__ void decode_append_kernel(uint8_t* k_cache, uint8_t* v_cache, long long row_stride_bytes,
                                      long long head_stride_bytes, const uint8_t* k_new, const uint8_t* v_new,
@@ -798,7 +878,7 @@ __global__ void decode_append_kernel(uint8_t* k_cache, uint8_t* v_cache, long lo
   uint8_t* dst = (blockIdx.y == 0 ? k_cache : v_cache) + cache_row * row_stride_bytes;
   const uint8_t* src = (blockIdx.y == 0 ? k_new : v_new) + in_row * hkv * row_bytes;
   const bool rotate = blockIdx.y == 0 && p.rotary_cos != nullptr;
-  const int pos = rotate ? rotary_pos(p, b, t) : 0;
+  const int pos = rotate ? rotary_pos(p, b, new_token_pos<true>(p, b, t, true)) : 0;
   const int chunks = row_bytes / 16;
   for (int idx = threadIdx.x; idx < hkv * chunks; idx += blockDim.x) {
     const int head = idx / chunks, c = idx % chunks;
@@ -825,7 +905,7 @@ __global__ void decode_append_e4m3_kernel(uint8_t* k_cache, uint8_t* v_cache, lo
   const T* src = (blockIdx.y == 0 ? k_new : v_new) + in_row * hkv * head_dim;
   const float* descale = (blockIdx.y == 0 ? p.k_descale : p.v_descale) + b * hkv;
   const bool rotate = blockIdx.y == 0 && p.rotary_cos != nullptr;
-  const int pos = rotate ? rotary_pos(p, b, t) : 0;
+  const int pos = rotate ? rotary_pos(p, b, new_token_pos<true>(p, b, t, true)) : 0;
   const int chunks = head_dim / 8;
   for (int idx = threadIdx.x; idx < hkv * chunks; idx += blockDim.x) {
     const int head = idx / chunks, c = idx % chunks;
@@ -906,6 +986,7 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
     if (new_dtype == kDtypeE4M3 && p.rotary_cos != nullptr) return "rotary needs a bf16 / fp16 k_new";
   }
   if (p.hkv <= 0 || p.hq % p.hkv != 0) return "query heads must be a multiple of kv heads";
+  if (p.tree_mask != nullptr && !p.causal) return "a tree mask replaces the causal rule: it needs causal";
   if (k_cache.row_stride != v_cache.row_stride || k_cache.head_stride != v_cache.head_stride)
     return "k_cache and v_cache must have the same strides";
   if (p.page_size != 0) {
@@ -965,28 +1046,35 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
     err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (err == cudaSuccess) kern<<<grid, threads, smem, stream>>>(tk, tv, p);
   };
-  auto pick = [&](auto t, auto f8) {
+  auto pick = [&](auto t, auto f8, auto tree) {
     using T = decltype(t);
-    constexpr bool kFp8 = decltype(f8)::value;
+    constexpr bool kFp8 = decltype(f8)::value, kTree = decltype(tree)::value;
     const int threads = kFp8 ? dec::kThreadsFp8 : dec::kThreads;
     if (head_dim == 128)
-      launch(dec::decode_kernel<T, 128, kFp8, false>, dec::smem_bytes<128, kFp8, false>(), threads);
-    else launch(dec::decode_kernel<T, 64, kFp8, false>, dec::smem_bytes<64, kFp8, false>(), threads);
-  };
-  if (q8) {  // e4m3 queries over an e4m3 cache: bf16 P V
-    if (head_dim == 128)
-      launch(dec::decode_kernel<__nv_bfloat16, 128, true, true>, dec::smem_bytes<128, true, true>(),
-             dec::kThreadsFp8);
+      launch(dec::decode_kernel<T, 128, kFp8, false, false, kTree>, dec::smem_bytes<128, kFp8, false, kTree>(),
+             threads);
     else
-      launch(dec::decode_kernel<__nv_bfloat16, 64, true, true>, dec::smem_bytes<64, true, true>(),
+      launch(dec::decode_kernel<T, 64, kFp8, false, false, kTree>, dec::smem_bytes<64, kFp8, false, kTree>(),
+             threads);
+  };
+  auto pick_q8 = [&](auto tree) {  // e4m3 queries over an e4m3 cache: bf16 P V
+    constexpr bool kTree = decltype(tree)::value;
+    if (head_dim == 128)
+      launch(dec::decode_kernel<__nv_bfloat16, 128, true, true, false, kTree>,
+             dec::smem_bytes<128, true, true, kTree>(), dec::kThreadsFp8);
+    else
+      launch(dec::decode_kernel<__nv_bfloat16, 64, true, true, false, kTree>, dec::smem_bytes<64, true, true, kTree>(),
              dec::kThreadsFp8);
-  } else if (dtype == kDtypeBF16) {
-    if (fp8) pick(__nv_bfloat16{}, std::true_type{});
-    else pick(__nv_bfloat16{}, std::false_type{});
-  } else {
-    if (fp8) pick(__half{}, std::true_type{});
-    else pick(__half{}, std::false_type{});
-  }
+  };
+  auto pick_cache = [&](auto tree) {
+    if (q8) pick_q8(tree);
+    else if (dtype == kDtypeBF16 && fp8) pick(__nv_bfloat16{}, std::true_type{}, tree);
+    else if (dtype == kDtypeBF16) pick(__nv_bfloat16{}, std::false_type{}, tree);
+    else if (fp8) pick(__half{}, std::true_type{}, tree);
+    else pick(__half{}, std::false_type{}, tree);
+  };
+  if (p.tree_mask != nullptr) pick_cache(std::true_type{});
+  else pick_cache(std::false_type{});
   if (err != cudaSuccess) return cudaGetErrorString(err);
   err = cudaGetLastError();
   return err == cudaSuccess ? nullptr : cudaGetErrorString(err);
@@ -1005,6 +1093,7 @@ const char* decode_prefix_launch(int dtype, int cache_dtype, const TensorView& k
       p.cache_leftpad != nullptr)
     return "the shared-prefix pass takes no q_descale, append, block table, cache slots or left pads";
   if (p.hkv <= 0 || p.hq % p.hkv != 0) return "query heads must be a multiple of kv heads";
+  if (p.tree_mask != nullptr && !p.causal) return "a tree mask replaces the causal rule: it needs causal";
   if (n_prefix < 1 || p.batch % n_prefix != 0 || p.prefix_n != p.batch / n_prefix)
     return "the batch must be prefix_n sequences per prefix";
   if (k_prefix.row_stride != v_prefix.row_stride || k_prefix.head_stride != v_prefix.head_stride)
@@ -1030,21 +1119,23 @@ const char* decode_prefix_launch(int dtype, int cache_dtype, const TensorView& k
     err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (err == cudaSuccess) kern<<<grid, threads, smem, stream>>>(tk, tv, p);
   };
-  auto pick = [&](auto t, auto f8) {
+  // the prefix pass masks nothing: a tree mask only moves its rotary positions
+  auto pick = [&](auto t, auto f8, auto tree) {
     using T = decltype(t);
-    constexpr bool kFp8 = decltype(f8)::value;
+    constexpr bool kFp8 = decltype(f8)::value, kTree = decltype(tree)::value;
     const int threads = kFp8 ? dec::kThreadsFp8 : dec::kThreads;
     if (head_dim == 128)
-      launch(dec::decode_kernel<T, 128, kFp8, false, true>, dec::smem_bytes<128, kFp8, false>(), threads);
-    else launch(dec::decode_kernel<T, 64, kFp8, false, true>, dec::smem_bytes<64, kFp8, false>(), threads);
+      launch(dec::decode_kernel<T, 128, kFp8, false, true, kTree>, dec::smem_bytes<128, kFp8, false>(), threads);
+    else launch(dec::decode_kernel<T, 64, kFp8, false, true, kTree>, dec::smem_bytes<64, kFp8, false>(), threads);
   };
-  if (dtype == kDtypeBF16) {
-    if (fp8) pick(__nv_bfloat16{}, std::true_type{});
-    else pick(__nv_bfloat16{}, std::false_type{});
-  } else {
-    if (fp8) pick(__half{}, std::true_type{});
-    else pick(__half{}, std::false_type{});
-  }
+  auto pick_cache = [&](auto tree) {
+    if (dtype == kDtypeBF16 && fp8) pick(__nv_bfloat16{}, std::true_type{}, tree);
+    else if (dtype == kDtypeBF16) pick(__nv_bfloat16{}, std::false_type{}, tree);
+    else if (fp8) pick(__half{}, std::true_type{}, tree);
+    else pick(__half{}, std::false_type{}, tree);
+  };
+  if (p.tree_mask != nullptr && p.rotary_cos != nullptr) pick_cache(std::true_type{});
+  else pick_cache(std::false_type{});
   if (err != cudaSuccess) return cudaGetErrorString(err);
   err = cudaGetLastError();
   return err == cudaSuccess ? nullptr : cudaGetErrorString(err);

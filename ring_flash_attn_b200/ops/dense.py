@@ -50,11 +50,13 @@ def block_fwd(
     scale: float,
     diag: Optional[int] = None,
     lo: Optional[int] = None,
+    mask: Optional[torch.Tensor] = None,
 ) -> Tuple[torch.Tensor, torch.Tensor]:
     """One (query chunk x key segment) block.  Returns (out fp32 (Tq,Hq,D), lse fp32 (Hq,Tq)).
 
-    Rows that see no key get ``out = 0`` and ``lse = -inf`` so that they are the identity of the
-    online-softmax merge (``ops/merge.py``).
+    ``mask``, optional, is an explicit boolean (Tq, Tk) mask (True = visible), applied together with
+    the ``diag`` / ``lo`` rule.  Rows that see no key get ``out = 0`` and ``lse = -inf`` so that they
+    are the identity of the online-softmax merge (``ops/merge.py``).
     """
     tq, hq, _ = q.shape
     tk, hkv, _ = k.shape
@@ -64,6 +66,8 @@ def block_fwd(
     vf = _expand_kv(v.float(), n_rep).transpose(0, 1)
     s = torch.matmul(qf, kf.transpose(1, 2)) * scale  # (Hq, Tq, Tk)
     m = diag_mask(tq, tk, diag, q.device, lo)
+    if mask is not None:
+        m = mask if m is None else m & mask
     if m is not None:
         s = s.masked_fill(~m, NEG_INF)
     lse = torch.logsumexp(s, dim=-1)  # (Hq, Tq); -inf for empty rows

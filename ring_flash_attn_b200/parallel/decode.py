@@ -135,7 +135,7 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
                   cache_leftpad: Optional[Tensor] = None, prefix_k_cache: Optional[Tensor] = None,
                   prefix_v_cache: Optional[Tensor] = None, prefix_seqlens: Optional[Tensor] = None,
                   prefix_k_descale: Optional[Tensor] = None, prefix_v_descale: Optional[Tensor] = None,
-                  prefix_splits: Optional[int] = None) -> Tuple[Tensor, Tensor]:
+                  prefix_splits: Optional[int] = None, tree_mask: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
     """Local split-KV kernel (appending ``k`` / ``v`` first when given), then the combine over the splits and, for
     ``world > 1``, over the gathered per-rank partials.  ``splits`` overrides :func:`num_splits`.  With
     ``block_table`` the caches are page pools (see :func:`cp_flash_attn_with_kvcache`).  e4m3 caches take contiguous
@@ -149,7 +149,10 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
     ``prefix_k_cache`` / ``prefix_v_cache`` ``(P, P_cap, Hkv, D)`` (contiguous), ``prefix_seqlens`` ``(P,)`` int32 and,
     for e4m3 caches, contiguous fp32 ``(P, Hkv)`` ``prefix_k_descale`` / ``prefix_v_descale``, a second kernel adds
     the attention of sequence ``b`` to prefix ``b // (B // P)``, in ``prefix_splits`` (default
-    :func:`num_splits_prefix`) more partial slabs that the same combine merges."""
+    :func:`num_splits_prefix`) more partial slabs that the same combine merges.  ``tree_mask`` (contiguous bool
+    ``(B, Sq, Sq)``, or ``(total_q, max_seqlen_q)`` when varlen; needs ``causal``) says which appended keys each new
+    token sees and sets the rotary positions of ``q`` and ``k`` (see :func:`cp_flash_attn_with_kvcache`); it is passed
+    on every rank."""
     C = cuda_ext.load()
     varlen = cu_seqlens_q is not None
     if varlen:  # the partials are the uniform layout at batch 1, Sq = total_q
@@ -185,6 +188,9 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
     extra = () if q_descale is None else (q_descale,)  # decode_fwd takes q_descale only for an e4m3 q
     if cache_batch_idx is not None or cache_leftpad is not None:
         extra = (q_descale, cache_batch_idx, cache_leftpad)
+    if tree_mask is not None:  # (rows, Sq): row = packed query row
+        tree_mask = tree_mask.view(-1, tree_mask.shape[-1])
+        extra = (q_descale, cache_batch_idx, cache_leftpad, tree_mask)
     C.decode_fwd(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, parts[:splits], block_table,
                  k_descale, v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0, rotary_cos, rotary_sin,
                  rotary_seqlens, bool(rotary_interleaved), *extra)
@@ -192,7 +198,8 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
     if prefix:  # the prefix partials go to the slabs after the suffix pass's
         C.decode_prefix_fwd(q, prefix_k_cache, prefix_v_cache, prefix_seqlens, causal, softmax_scale, parts[splits:],
                             prefix_k_descale, prefix_v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0,
-                            rotary_cos, rotary_sin, rotary_seqlens, bool(rotary_interleaved))
+                            rotary_cos, rotary_sin, rotary_seqlens, bool(rotary_interleaved),
+                            *(() if tree_mask is None else (tree_mask,)))
         cuda_ext.note_launch()
     if world > 1:
         mine = torch.empty(size, dtype=torch.float32, device=q.device)
@@ -235,12 +242,30 @@ def apply_rotary(x: Tensor, cos: Tensor, sin: Tensor, positions: Tensor, interle
     return torch.cat([y.to(x.dtype), x[..., 2 * h:]], dim=-1)
 
 
-def _rotary_positions(rotary_seqlens: Tensor, spans, seqlen_ro: int, causal: bool, device):
+def tree_depths(tree_mask: Tensor, spans) -> list:
+    """Per packed new token, its depth: the True entries among the first ``n_b`` of its ``(rows, Sq)`` tree-mask row,
+    minus one (0 for an empty row).  The rotary offset of a new token with a tree mask."""
+    depths = []
+    for lo, n in spans:
+        depths += (tree_mask[lo:lo + n, :n].sum(1) - 1).clamp(min=0).tolist()
+    return depths
+
+
+def _rotary_positions(rotary_seqlens: Tensor, spans, seqlen_ro: int, causal: bool, device, depths=None):
     """Table rows of the packed new tokens, (keys, queries): key t of sequence b at ``rotary_seqlens[b] + t``, query
-    token t there too when causal, at ``rotary_seqlens[b]`` otherwise.  ``ValueError`` for a position outside the
-    tables (the kernel clamps instead)."""
+    token t there too when causal, at ``rotary_seqlens[b]`` otherwise; with a tree mask both at
+    ``rotary_seqlens[b] + depths[row]``.  ``ValueError`` for a position outside the tables (the kernel clamps
+    instead)."""
     keys, queries = [], []
-    for i, (start, (_, n)) in enumerate(zip(rotary_seqlens.tolist(), spans)):
+    for i, (start, (lo, n)) in enumerate(zip(rotary_seqlens.tolist(), spans)):
+        if depths is not None:
+            pos = [start + x for x in depths[lo:lo + n]]
+            if pos and not (0 <= min(pos) and max(pos) < seqlen_ro):
+                raise ValueError(f"rotary positions [{min(pos)}, {max(pos)}] of sequence {i} are outside the "
+                                 f"{seqlen_ro}-row rotary tables")
+            keys += pos
+            queries += pos
+            continue
         if n and not 0 <= start <= seqlen_ro - n:
             raise ValueError(f"rotary positions [{start}, {start + n}) of sequence {i} are outside the "
                              f"{seqlen_ro}-row rotary tables")
@@ -265,7 +290,7 @@ def _varlen_spans(cu_seqlens_q: Tensor, total_q: int, max_seqlen_q: int):
 
 def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table=None,
                   k_descale=None, v_descale=None, cu_seqlens_q=None, max_seqlen_q=0, rotary=None, q_descale=None,
-                  cache_batch_idx=None, cache_leftpad=None, prefix=None):
+                  cache_batch_idx=None, cache_leftpad=None, prefix=None, tree_mask=None):
     # every sequence is a (first row, count) span of the packed rows: (b * Sq, Sq) for a uniform q
     out_dtype = _out_dtype(q)
     b = cache_seqlens.shape[0]
@@ -280,7 +305,8 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
             k, v = k.reshape(b * sq, *k.shape[2:]), v.reshape(b * sq, *v.shape[2:])
     if rotary is not None:  # (cos, sin, rotary_seqlens, interleaved): q on every rank, k where it is appended
         cos, sin, rotary_seqlens, interleaved = rotary
-        key_pos, q_pos = _rotary_positions(rotary_seqlens, spans, cos.shape[0], causal, q.device)
+        depths = None if tree_mask is None else tree_depths(tree_mask, spans)
+        key_pos, q_pos = _rotary_positions(rotary_seqlens, spans, cos.shape[0], causal, q.device, depths)
         q = apply_rotary(q, cos, sin, q_pos, interleaved)
         if k is not None:
             k = apply_rotary(k, cos, sin, key_pos, interleaved)
@@ -354,9 +380,13 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
                 pkk, pvv = pkk.float() * pkd[p][:, None], pvv.float() * pvd[p][:, None]
             kk, vv = torch.cat([pkk.to(kk.dtype), kk]), torch.cat([pvv.to(vv.dtype), vv])
         # appended key u (row n + u) is visible to token t iff u <= t, i.e. row j <= t + n (j counted from lp, after
-        # the prefix rows)
-        diag = n_pre + n - lp if (n_new and causal) else None
-        out[lo:lo + cnt], lse[:, lo:lo + cnt] = block_fwd(q[lo:lo + cnt], kk, vv, softmax_scale, diag)
+        # the prefix rows); with a tree mask iff tree_mask[lo + t, u], every earlier row staying visible
+        diag = n_pre + n - lp if (n_new and causal and tree_mask is None) else None
+        mask = None
+        if n_new and tree_mask is not None:
+            mask = torch.cat([torch.ones(cnt, n_pre + n - lp, dtype=torch.bool, device=q.device),
+                              tree_mask[lo:lo + cnt, :n_keys - n]], dim=1)
+        out[lo:lo + cnt], lse[:, lo:lo + cnt] = block_fwd(q[lo:lo + cnt], kk, vv, softmax_scale, diag, mask=mask)
     if world > 1:
         parts = _gather(torch.cat([out.reshape(-1), lse.reshape(-1)]), pg, world)
         n_out = out.numel()
@@ -385,7 +415,7 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
               cache_batch_idx: Optional[Tensor] = None, cache_leftpad: Optional[Tensor] = None,
               prefix_k_cache: Optional[Tensor] = None, prefix_v_cache: Optional[Tensor] = None,
               prefix_seqlens: Optional[Tensor] = None, prefix_k_descale: Optional[Tensor] = None,
-              prefix_v_descale: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+              prefix_v_descale: Optional[Tensor] = None, tree_mask: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
     """q (B, Sq, Hq, D) -> (out (B, Sq, Hq, D) in q.dtype (bf16 for an e4m3 q), lse (B, Hq, Sq) fp32).  ``k`` /
     ``v`` are appended to the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's
     name ("" = world); with ``block_table`` the caches are this rank's page pools; e4m3 caches come with contiguous
@@ -395,7 +425,9 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
     it stores it.  An e4m3 q comes with a contiguous fp32 (B, Hkv) ``q_descale``.  ``cache_batch_idx`` /
     ``cache_leftpad`` (B,) int32 pick each sequence's cache slot and first key row.  ``prefix_k_cache`` /
     ``prefix_v_cache`` (P, P_cap, Hkv, D) with ``prefix_seqlens`` (P,) int32 (and fp32 (P, Hkv) descales for e4m3)
-    are this rank's shards of the prefixes shared by consecutive groups of B / P sequences (read-only)."""
+    are this rank's shards of the prefixes shared by consecutive groups of B / P sequences (read-only).  ``tree_mask``
+    (B, Sq, Sq) bool, or (total_q, max_seqlen_q) when varlen, says which appended keys each new token sees; it is
+    passed on every rank, since it also sets the rotary positions of q."""
     pg = resolve_group(group)
     rank, world = group_info(pg)
     if k is not None and not 0 <= append_rank < world:
@@ -411,20 +443,20 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
                              cache_batch_idx=cache_batch_idx, cache_leftpad=cache_leftpad,
                              prefix_k_cache=prefix_k_cache, prefix_v_cache=prefix_v_cache,
                              prefix_seqlens=prefix_seqlens, prefix_k_descale=prefix_k_descale,
-                             prefix_v_descale=prefix_v_descale)
+                             prefix_v_descale=prefix_v_descale, tree_mask=tree_mask)
     rotary = None if rotary_cos is None else (rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved)
     prefix = None if prefix_k_cache is None else (prefix_k_cache, prefix_v_cache, prefix_seqlens, prefix_k_descale,
                                                   prefix_v_descale)
     return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table,
                          k_descale, v_descale, cu_seqlens_q, max_seqlen_q, rotary, q_descale, cache_batch_idx,
-                         cache_leftpad, prefix)
+                         cache_leftpad, prefix, None if tree_mask is None else tree_mask.view(-1, tree_mask.shape[-1]))
 
 
 @cp_decode.register_fake
 def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group, block_table, k_descale,
       v_descale, cu_seqlens_q, max_seqlen_q, rotary_cos=None, rotary_sin=None, rotary_seqlens=None,
       rotary_interleaved=True, q_descale=None, cache_batch_idx=None, cache_leftpad=None, prefix_k_cache=None,
-      prefix_v_cache=None, prefix_seqlens=None, prefix_k_descale=None, prefix_v_descale=None):
+      prefix_v_cache=None, prefix_seqlens=None, prefix_k_descale=None, prefix_v_descale=None, tree_mask=None):
     out = q.new_empty(q.shape, dtype=_out_dtype(q))
     if cu_seqlens_q is not None:
         total_q, hq, _ = q.shape
@@ -552,13 +584,32 @@ def _check_rotary(cos, sin, rotary_seqlens, q, b, d, cache_seqlens, group):
     return rotary_seqlens
 
 
+MAX_TREE_TOKENS = 128  # new tokens per sequence with a tree mask: they span at most two key tiles
+
+
+def _check_tree_mask(tree_mask, q, k, causal, shape):
+    if k is None:
+        raise ValueError("tree_mask needs k / v: it says which of the keys this call appends each new token sees")
+    if not causal:
+        raise ValueError("tree_mask replaces the causal rule among the appended keys: it needs causal=True")
+    if not isinstance(tree_mask, Tensor) or tree_mask.dtype != torch.bool:
+        raise ValueError("tree_mask must be a torch.bool tensor")
+    if tuple(tree_mask.shape) != tuple(shape) or not tree_mask.is_contiguous():
+        raise ValueError(f"tree_mask must be contiguous with shape {tuple(shape)} ((B, Sq, Sq), or (total_q, "
+                         f"max_seqlen_q) with cu_seqlens_q), not {tuple(tree_mask.shape)}")
+    if tree_mask.device != q.device:
+        raise ValueError("tree_mask must be on q's device")
+    if shape[-1] > MAX_TREE_TOKENS:
+        raise ValueError(f"tree_mask takes at most {MAX_TREE_TOKENS} new tokens per sequence, not {shape[-1]}")
+
+
 def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=None, append_rank=None,
                                softmax_scale=None, causal=True, return_softmax_lse=False, group=None, *,
                                block_table=None, k_descale=None, v_descale=None, cu_seqlens_q=None,
                                max_seqlen_q=None, rotary_cos=None, rotary_sin=None, rotary_interleaved=True,
                                rotary_seqlens=None, window_size=(-1, -1), alibi_slopes=None, q_descale=None,
                                cache_batch_idx=None, cache_leftpad=None, prefix_k_cache=None, prefix_v_cache=None,
-                               prefix_seqlens=None, prefix_k_descale=None, prefix_v_descale=None):
+                               prefix_seqlens=None, prefix_k_descale=None, prefix_v_descale=None, tree_mask=None):
     """Decode attention of new query tokens against a KV cache sharded over ``group`` (modelled on flash-attn's
     ``flash_attn_with_kvcache``).  Inference only: no gradient.
 
@@ -652,6 +703,22 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
       access outside ``q``, ``k``, ``v`` or the caches.  The dense path raises ``ValueError`` for them
       (``cu_seqlens_q[0] != 0``, a decreasing entry, ``cu_seqlens_q[B] != total_q``, a count above
       ``max_seqlen_q``).  Long chunks are correct but not efficient: every 64-row tile reads the whole shard.
+    * Tree attention (speculative decoding: EAGLE, Medusa and other draft trees verified in one call):
+      ``tree_mask``, a contiguous ``torch.bool`` tensor on q's device, the same on every rank, of shape
+      ``(B, Sq, Sq)``, or ``(total_q, max_seqlen_q)`` with ``cu_seqlens_q``.  Its rows are the packed query rows and
+      column ``u`` is new key ``u`` of the row's own sequence (in a varlen call columns at or past ``n_b`` are
+      ignored): new token ``t`` of sequence ``b`` sees appended key ``u`` iff ``tree_mask[row(b, t), u]``.  This
+      replaces the causal rule among the appended keys only; every valid cached key (own cache, prefix, pages, slots,
+      left pad) stays visible to every new token.  Any boolean matrix is accepted; a tree's ancestor mask (ancestors
+      plus the node itself) is the intended use, and a lower-triangular mask gives exactly the causal call.  It needs
+      ``k`` / ``v``, ``causal=True`` and at most 128 new tokens per sequence.  With rotary, new token ``t`` (query and
+      key) sits at ``rotary_seqlens[b] + max(n_t - 1, 0)``, ``n_t`` being the True entries of its row: a node's depth
+      in a tree, and ``t`` for a lower-triangular mask.  Node ``u`` is still appended at row
+      ``cache_seqlens[b] + u`` of the append rank; keeping the accepted nodes (moving their rows to
+      ``cache_seqlens[b] + [0, n_accepted)``) and advancing ``cache_seqlens`` is the caller's job.  The kernel path
+      reads the mask on the device only and never validates it, so a CUDA graph replay uses its current contents.
+      Masks over cached keys, a mask without ``causal`` and bit-packed masks are not supported; a wrong dtype,
+      shape, device or contiguity raises ``ValueError``.
     * Returns ``out`` ``(B, Sq, Hq, D)`` in q.dtype (bf16 for an e4m3 ``q``), and ``softmax_lse`` ``(B, Hq, Sq)``
       fp32 when ``return_softmax_lse``.  Both are bitwise identical on every rank.
     * ``window_size``, ``alibi_slopes``, ``D > 128`` and ``Hq % Hkv != 0`` raise ``ValueError``.  The sm_90a kernel
@@ -796,10 +863,12 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
             raise ValueError("rotary_cos / rotary_sin need k / v: the rotation applies to the new tokens")
     elif rotary_seqlens is not None:
         raise ValueError("rotary_seqlens is only taken with rotary_cos / rotary_sin")
+    if tree_mask is not None:
+        _check_tree_mask(tree_mask, q, k, causal, (total_q, sq) if varlen else (b, sq, sq))
     scale = float(softmax_scale) if softmax_scale is not None else d ** -0.5
     out, lse = cp_decode(q, k_cache, v_cache, cache_seqlens, k, v, -1 if append_rank is None else int(append_rank),
                          scale, bool(causal), group_name(group), block_table, k_descale, v_descale, cu_seqlens_q,
                          max_seqlen_q if varlen else 0, rotary_cos, rotary_sin, rotary_seqlens,
                          bool(rotary_interleaved), q_descale, cache_batch_idx, cache_leftpad, prefix_k_cache,
-                         prefix_v_cache, prefix_seqlens, prefix_k_descale, prefix_v_descale)
+                         prefix_v_cache, prefix_seqlens, prefix_k_descale, prefix_v_descale, tree_mask)
     return (out, lse) if return_softmax_lse else out
