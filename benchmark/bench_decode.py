@@ -31,12 +31,14 @@ the slot and plain outputs are bitwise equal.  With ``--leftpad P`` it also time
 pad rows below their keys (``cache_leftpad``) against the plain call on the same number of valid rows.  Both arms run
 over the cache and query dtypes that ``--kv-dtype`` / ``--q-dtype`` select.
 With ``--shared-prefix L --samples n`` the run times shared-prefix decoding instead: P prompts (``--prompts``) of L
-tokens per rank, n samples each, every sample with its own ``--suffix`` rows and one appended token per call, in three
+tokens per rank, n samples each, every sample with its own ``--suffix`` rows and one appended token per call, in four
 arms with the same contents, alternating in one loop: the prefix call (``prefix_k_cache`` / ``prefix_v_cache``), the
-prompt copied into each sample's contiguous cache ahead of its suffix (a plain call), and paged caches of 128-row pages
-whose block tables share the prompt's pages.  Each line reports the HBM bytes each arm must read (from shapes), the
-largest difference between the arms' outputs, and the card's name, power limit and maximum SM clock (read in one
-``nvidia-smi`` query).  ``--kv-dtype e4m3`` runs the three arms over e4m3 caches with one descale per kv head.
+prompt copied into each sample's contiguous cache ahead of its suffix (a plain call), paged caches of
+``--prefix-page``-row pages (128 by default) whose block tables share the prompt's pages, and the paged prefix call on
+that same pool (``prefix_block_table`` names the prompt's pages, ``block_table`` each sample's own).  Each line reports
+the HBM bytes each arm must read (from shapes), the largest difference between the arms' outputs, whether the paged
+prefix call's out / lse are bitwise the prefix call's, and the card's name, power limit and maximum SM clock (read in
+one ``nvidia-smi`` query).  ``--kv-dtype e4m3`` runs the four arms over e4m3 caches with one descale per kv head.
 With ``--tree W1,W2,...`` the run times speculative-tree verification instead: a full draft tree in which every node
 at depth i has Wi children (plus the root; ``4,2,2,1`` has 45 nodes and 16 leaves), one per sequence, against caches
 of ``--cache`` tokens, in three arms alternating in one loop, each appending its tokens: the tree call (``tree_mask``,
@@ -55,6 +57,7 @@ in the tree call and the same node's row in a per-path call, and the card's name
     python benchmark/bench_decode.py --leftpad 1000       # also a left-padded call against the plain one
     torchrun --nproc-per-node 2 benchmark/bench_decode.py
     python benchmark/bench_decode.py --shared-prefix 32768 131072 --samples 4 16   # one prompt, n samples
+    python benchmark/bench_decode.py --shared-prefix 32768 --prefix-page 16        # the paged arms in pages of 16
     python benchmark/bench_decode.py --tree 4,2,2,1       # a 45-node draft tree: tree vs chain vs per-path calls
     python benchmark/bench_decode.py --dry-run            # shapes and byte counts only (no GPU)
 """
@@ -105,6 +108,8 @@ def parse_args(argv=None):
     ap.add_argument("--samples", type=int, nargs="+", default=[4, 16], help="samples per prompt (--shared-prefix)")
     ap.add_argument("--prompts", type=int, nargs="+", default=[1], help="prompts P per call (--shared-prefix)")
     ap.add_argument("--suffix", type=int, default=256, help="each sample's own cached rows (--shared-prefix)")
+    ap.add_argument("--prefix-page", type=int, default=PREFIX_PAGE,
+                    help="rows per page of the paged and paged-prefix arms (--shared-prefix)")
     ap.add_argument("--tree", type=str, default=None, metavar="W1,W2,...",
                     help="time tree verification instead: a full tree with Wi children per node at depth i")
     ap.add_argument("--dry-run", action="store_true")
@@ -119,6 +124,10 @@ def parse_args(argv=None):
     if args.shared_prefix is not None and (min(args.shared_prefix) < 1 or args.suffix < 1 or min(args.samples) < 1
                                            or min(args.prompts) < 1):
         ap.error("--shared-prefix, --samples, --prompts and --suffix must be positive")
+    if args.shared_prefix is not None and not dec._valid_page_size(args.prefix_page):
+        ap.error("--prefix-page must be 16, 32, 64 or a positive multiple of 128")
+    if args.shared_prefix is not None and min(x % args.prefix_page for x in args.shared_prefix) != 0:
+        ap.error("--shared-prefix must be a multiple of --prefix-page for the paged arms")
     if args.cache_slots is not None and args.cache_slots < max(args.batch):
         ap.error("--cache-slots must be at least the largest --batch (the sequences use distinct slots)")
     if args.leftpad is not None and not 0 <= args.leftpad < min(args.cache):
@@ -166,7 +175,7 @@ def shapes(args, sm_count):
             yield cfg
 
 
-PREFIX_PAGE = 128  # rows per page of the paged arm
+PREFIX_PAGE = 128  # rows per page of the paged and paged-prefix arms, unless --prefix-page says otherwise
 
 
 def prefix_shapes(args, sm_count):
@@ -180,13 +189,14 @@ def prefix_shapes(args, sm_count):
                 b, suf = n_prompts * n, args.suffix
                 slots = dec.prefix_tile_slots(n, 1, args.hq, hkv)
                 yield dict(shared_prefix=length, samples=n, prompts=n_prompts, batch=b, suffix=suf, sq=1, hq=args.hq,
-                           hkv=hkv, head_dim=d, kv_dtype=args.kv_dtype, page_size=PREFIX_PAGE,
+                           hkv=hkv, head_dim=d, kv_dtype=args.kv_dtype, page_size=args.prefix_page,
                            suffix_splits=dec.num_splits(b, 1, args.hq, hkv, suf, sm_count),
                            prefix_splits=dec.num_splits_prefix(n_prompts, slots, hkv, length, sm_count),
                            plain_splits=dec.num_splits(b, 1, args.hq, hkv, length + suf, sm_count),
                            rows_per_prefix_tile=min(n * g, dec.ROWS_PER_CTA),
                            prefix_bytes=(n_prompts * length + b * suf) * row,
-                           copied_bytes=b * (length + suf) * row, paged_bytes=b * (length + suf) * row)
+                           copied_bytes=b * (length + suf) * row, paged_bytes=b * (length + suf) * row,
+                           paged_prefix_bytes=(n_prompts * length + b * suf) * row)
 
 
 def card_settings():
@@ -201,7 +211,7 @@ def card_settings():
 
 
 def shared_prefix_main(args):
-    """The three shared-prefix arms, alternating in one loop (see the module docstring)."""
+    """The four shared-prefix arms, alternating in one loop (see the module docstring)."""
     if args.dry_run:
         for cfg in prefix_shapes(args, args.sm_count):
             print(json.dumps(cfg))
@@ -243,23 +253,22 @@ def shared_prefix_main(args):
         ck = torch.cat([raw(pk)[owner], raw(sk)], dim=1).view(pk.dtype)
         cv = torch.cat([raw(pv)[owner], raw(sv)], dim=1).view(pv.dtype)
         # paged: the prompt's pages once per prompt, then each sample's own pages; the tables share the prompt pages
-        p_pages, s_pages = -(-length // PREFIX_PAGE), -(-suf // PREFIX_PAGE)
-        assert length % PREFIX_PAGE == 0, "--shared-prefix must be a multiple of 128 for the paged arm"
+        ps = cfg["page_size"]
+        p_pages, s_pages = length // ps, -(-suf // ps)
 
         def pool_of(pre, own):
             rb = d * pre.element_size()  # bytes per (row, kv head)
-            pool = torch.zeros((n_prompts * p_pages + b * s_pages, PREFIX_PAGE, hkv, rb), dtype=torch.uint8,
-                               device=dev)
-            pool[:n_prompts * p_pages] = raw(pre).reshape(n_prompts * p_pages, PREFIX_PAGE, hkv, rb)
-            padded = torch.zeros((b, s_pages * PREFIX_PAGE, hkv, rb), dtype=torch.uint8, device=dev)
+            pool = torch.zeros((n_prompts * p_pages + b * s_pages, ps, hkv, rb), dtype=torch.uint8, device=dev)
+            pool[:n_prompts * p_pages] = raw(pre).reshape(n_prompts * p_pages, ps, hkv, rb)
+            padded = torch.zeros((b, s_pages * ps, hkv, rb), dtype=torch.uint8, device=dev)
             padded[:, :suf] = raw(own)
-            pool[n_prompts * p_pages:] = padded.view(b * s_pages, PREFIX_PAGE, hkv, rb)
+            pool[n_prompts * p_pages:] = padded.view(b * s_pages, ps, hkv, rb)
             return pool.view(pre.dtype)
 
         gk, gv = pool_of(pk, sk), pool_of(pv, sv)
-        table = torch.cat([owner[:, None] * p_pages + torch.arange(p_pages, device=dev)[None],
-                           n_prompts * p_pages + torch.arange(b * s_pages, device=dev).view(b, s_pages)],
-                          dim=1).to(torch.int32)
+        prompt_table = torch.arange(n_prompts * p_pages, device=dev, dtype=torch.int32).view(n_prompts, p_pages)
+        own_table = (n_prompts * p_pages + torch.arange(b * s_pages, device=dev)).view(b, s_pages).to(torch.int32)
+        table = torch.cat([prompt_table[owner], own_table], dim=1)
 
         def prefix_call():
             return dec.kernel_decode(q, sk, sv, sl_own, k_new, v_new, True, scale, prefix_k_cache=pk,
@@ -271,7 +280,12 @@ def shared_prefix_main(args):
         def paged_call():
             return dec.kernel_decode(q, gk, gv, sl_all, k_new, v_new, True, scale, block_table=table, **kw)
 
-        arms = {"prefix": prefix_call, "copied": copied_call, "paged": paged_call}
+        def paged_prefix_call():  # one pool: the prompt's pages by prefix_block_table, the samples' by block_table
+            return dec.kernel_decode(q, gk, gv, sl_own, k_new, v_new, True, scale, block_table=own_table,
+                                     prefix_k_cache=gk, prefix_v_cache=gv, prefix_block_table=prompt_table,
+                                     prefix_seqlens=pl, **kw, **pkw)
+
+        arms = {"prefix": prefix_call, "copied": copied_call, "paged": paged_call, "paged_prefix": paged_prefix_call}
         times = {k: [] for k in arms}
         for _ in range(5):  # alternate them in one run
             for k, fn in arms.items():
@@ -284,11 +298,18 @@ def shared_prefix_main(args):
             res[f"{k}_GBps"] = round(cfg[f"{k}_bytes"] / (us * 1e-6) / 1e9, 1)
         res["prefix_speedup_vs_copied"] = round(res["copied_us"] / res["prefix_us"], 3)
         res["prefix_speedup_vs_paged"] = round(res["paged_us"] / res["prefix_us"], 3)
-        outs = {k: fn()[0].float() for k, fn in arms.items()}
+        res["paged_prefix_speedup_vs_copied"] = round(res["copied_us"] / res["paged_prefix_us"], 3)
+        res["paged_prefix_speedup_vs_paged"] = round(res["paged_us"] / res["paged_prefix_us"], 3)
+        res["paged_prefix_time_vs_prefix"] = round(res["paged_prefix_us"] / res["prefix_us"], 4)
+        results = {k: fn() for k, fn in arms.items()}
+        outs = {k: r[0].float() for k, r in results.items()}
         res["max_abs_diff_prefix_vs_copied"] = (outs["prefix"] - outs["copied"]).abs().max().item()
         res["max_abs_diff_paged_vs_copied"] = (outs["paged"] - outs["copied"]).abs().max().item()
+        res["max_abs_diff_paged_prefix_vs_copied"] = (outs["paged_prefix"] - outs["copied"]).abs().max().item()
+        res["paged_prefix_bitwise_prefix"] = bool(torch.equal(results["paged_prefix"][0], results["prefix"][0])
+                                                  and torch.equal(results["paged_prefix"][1], results["prefix"][1]))
         print(json.dumps(res), flush=True)
-        del q, k_new, v_new, pk, pv, sk, sv, ck, cv, gk, gv, outs
+        del q, k_new, v_new, pk, pv, sk, sv, ck, cv, gk, gv, outs, results
         torch.cuda.empty_cache()
 
 

@@ -614,14 +614,18 @@ void decode_fwd(const at::Tensor& q_in, at::Tensor& k_cache, at::Tensor& v_cache
 // mergeable first two dimensions, in q's dtype or both e4m3 with k_descale / v_descale fp32 (P, Hkv) contiguous.
 // Sequence b reads prefix b / (B / P), rows [0, prefix_seqlens[p]) (read on the device only, clamped to [0, P_cap]),
 // all visible to every query token.  part: the partial slabs of this pass, in decode_fwd's layout.  causal and the
-// rotary tensors position q's rotation as in decode_fwd, and so does tree_mask (which masks no prefix key).
+// rotary tensors position q's rotation as in decode_fwd, and so does tree_mask (which masks no prefix key).  With
+// prefix_block_table (P, max_prefix_blocks) int32, prefix_k / prefix_v are page pools (num_blocks, page_size, Hkv, D)
+// with mergeable page and row dimensions (they may be decode_fwd's own pools), row j of prefix p lives at row
+// j % page_size of page prefix_block_table[p, j / page_size], and P_cap = max_prefix_blocks * page_size.
 void decode_prefix_fwd(const at::Tensor& q_in, const at::Tensor& prefix_k, const at::Tensor& prefix_v,
                        const at::Tensor& prefix_seqlens, bool causal, double scale, at::Tensor& part,
                        const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale,
                        const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q,
                        const c10::optional<at::Tensor>& rotary_cos, const c10::optional<at::Tensor>& rotary_sin,
                        const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved,
-                       const c10::optional<at::Tensor>& tree_mask) {
+                       const c10::optional<at::Tensor>& tree_mask,
+                       const c10::optional<at::Tensor>& prefix_block_table) {
   const c10::cuda::CUDAGuard guard(q_in.device());
   const bool varlen = cu_seqlens_q.has_value();
   TORCH_CHECK(q_in.dim() == (varlen ? 3 : 4), "decode_prefix_fwd: q must be (B, Sq, Hq, D), or (total_q, Hq, D) "
@@ -641,8 +645,25 @@ void decode_prefix_fwd(const at::Tensor& q_in, const at::Tensor& prefix_k, const
   const int64_t sq = varlen ? max_seqlen_q : q.size(1), hq = q.size(2), d = q.size(3);
   const int64_t rows = varlen ? total_q : B * sq;
   TORCH_CHECK(prefix_k.dim() == 4 && prefix_k.sizes() == prefix_v.sizes(),
-              "decode_prefix_fwd: prefix_k / prefix_v must be the same (P, P_cap, Hkv, D) shape");
-  const int64_t n_prefix = prefix_k.size(0), p_cap = prefix_k.size(1), hkv = prefix_k.size(2);
+              "decode_prefix_fwd: prefix_k / prefix_v must be the same (P, P_cap, Hkv, D) shape, or the same "
+              "(num_blocks, page_size, Hkv, D) shape with prefix_block_table");
+  const bool paged = prefix_block_table.has_value();
+  const int64_t page_size = paged ? prefix_k.size(1) : 0;
+  const int64_t n_prefix = paged ? prefix_block_table->size(0) : prefix_k.size(0);
+  const int64_t p_cap = paged ? prefix_block_table->size(1) * page_size : prefix_k.size(1);
+  const int64_t hkv = prefix_k.size(2);
+  const int64_t cache_rows = prefix_k.size(0) * prefix_k.size(1);  // a contiguous cache's P * P_cap
+  if (paged) {
+    const at::Tensor& bt = *prefix_block_table;
+    TORCH_CHECK(bt.scalar_type() == at::kInt && bt.is_cuda() && bt.device() == q_in.device() && bt.dim() == 2 &&
+                    bt.size(0) >= 1 && bt.size(1) >= 1 && bt.stride(1) == 1,
+                "decode_prefix_fwd: prefix_block_table must be (P, max_prefix_blocks) int32 on q's device with "
+                "stride(1) == 1");
+    TORCH_CHECK(page_size == 16 || page_size == 32 || page_size == 64 || (page_size > 0 && page_size % 128 == 0),
+                "decode_prefix_fwd: page_size must be 16, 32, 64 or a positive multiple of 128");
+    TORCH_CHECK(cache_rows < (int64_t(1) << 31) && p_cap < (int64_t(1) << 31),
+                "decode_prefix_fwd: num_blocks * page_size and max_prefix_blocks * page_size must be below 2^31");
+  }
   const bool fp8 = prefix_k.scalar_type() == at::kFloat8_e4m3fn;
   TORCH_CHECK(prefix_k.scalar_type() == prefix_v.scalar_type() && (fp8 || prefix_k.scalar_type() == q.scalar_type()),
               "decode_prefix_fwd: the prefix caches must both have q's dtype or both be fp8 (float8_e4m3fn)");
@@ -650,7 +671,7 @@ void decode_prefix_fwd(const at::Tensor& q_in, const at::Tensor& prefix_k, const
               "decode_prefix_fwd: fp8 prefix caches need k_descale and v_descale, and other caches take none");
   TORCH_CHECK(n_prefix >= 1 && B % n_prefix == 0 && prefix_k.size(3) == d && hkv >= 1 && hq % hkv == 0,
               "decode_prefix_fwd: the prefix caches do not match q (P must divide B)");
-  TORCH_CHECK(n_prefix * p_cap < (int64_t(1) << 31), "decode_prefix_fwd: P * P_cap must be below 2^31");
+  TORCH_CHECK(paged || cache_rows < (int64_t(1) << 31), "decode_prefix_fwd: P * P_cap must be below 2^31");
   TORCH_CHECK(q.stride(3) == 1 && (varlen || q.stride(0) == sq * q.stride(1)),
               "decode_prefix_fwd: q must be (B, Sq) mergeable");
   TORCH_CHECK((q.stride(1) * q.element_size()) % 16 == 0 && (q.stride(2) * q.element_size()) % 16 == 0 &&
@@ -688,6 +709,12 @@ void decode_prefix_fwd(const at::Tensor& q_in, const at::Tensor& prefix_k, const
   p.causal = causal ? 1 : 0;
   p.scale_log2 = static_cast<float>(scale * 1.4426950408889634);
   p.prefix_n = static_cast<int>(B / n_prefix);
+  if (paged) {
+    p.block_table = prefix_block_table->data_ptr<int>();
+    p.bt_stride = prefix_block_table->stride(0);
+    p.page_size = static_cast<int>(page_size);
+    p.num_pages = static_cast<int>(prefix_k.size(0));
+  }
   if (fp8) {
     for (const at::Tensor* t : {&*k_descale, &*v_descale})
       TORCH_CHECK(t->scalar_type() == at::kFloat && t->device() == q.device() && t->dim() == 2 &&
@@ -721,7 +748,6 @@ void decode_prefix_fwd(const at::Tensor& q_in, const at::Tensor& prefix_k, const
     p.rotary_interleaved = rotary_interleaved ? 1 : 0;
   }
   p.tree_mask = tree_mask_ptr(tree_mask, q, rows, sq, causal, "decode_prefix_fwd");
-  const int64_t cache_rows = n_prefix * p_cap;
   const TensorView kv{prefix_k.data_ptr(), cache_rows, static_cast<int>(hkv), prefix_k.stride(1), prefix_k.stride(2)};
   const TensorView vv{prefix_v.data_ptr(), cache_rows, static_cast<int>(hkv), prefix_v.stride(1), prefix_v.stride(2)};
   check(rfa::decode_prefix_launch(dtype_code(q), fp8 ? rfa::kDtypeE4M3 : dtype_code(q), kv, vv, p,
@@ -834,6 +860,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                c10::nullopt, c10::nullopt, c10::nullopt);
   });
   m.def("decode_prefix_fwd", &decode_prefix_fwd);
+  // the same without prefix_block_table (a contiguous prefix)
+  m.def("decode_prefix_fwd", [](const at::Tensor& q, const at::Tensor& prefix_k, const at::Tensor& prefix_v,
+                                const at::Tensor& prefix_seqlens, bool causal, double scale, at::Tensor& part,
+                                const c10::optional<at::Tensor>& k_descale, const c10::optional<at::Tensor>& v_descale,
+                                const c10::optional<at::Tensor>& cu_seqlens_q, int64_t max_seqlen_q,
+                                const c10::optional<at::Tensor>& rotary_cos,
+                                const c10::optional<at::Tensor>& rotary_sin,
+                                const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved,
+                                const c10::optional<at::Tensor>& tree_mask) {
+    decode_prefix_fwd(q, prefix_k, prefix_v, prefix_seqlens, causal, scale, part, k_descale, v_descale, cu_seqlens_q,
+                      max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, tree_mask,
+                      c10::nullopt);
+  });
   // the same without tree_mask
   m.def("decode_prefix_fwd", [](const at::Tensor& q, const at::Tensor& prefix_k, const at::Tensor& prefix_v,
                                 const at::Tensor& prefix_seqlens, bool causal, double scale, at::Tensor& part,
@@ -843,7 +882,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
                                 const c10::optional<at::Tensor>& rotary_sin,
                                 const c10::optional<at::Tensor>& rotary_seqlens, bool rotary_interleaved) {
     decode_prefix_fwd(q, prefix_k, prefix_v, prefix_seqlens, causal, scale, part, k_descale, v_descale, cu_seqlens_q,
-                      max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, c10::nullopt);
+                      max_seqlen_q, rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved, c10::nullopt,
+                      c10::nullopt);
   });
   m.def("decode_combine", &decode_combine);
   rfa::bind_peer_mem(m);

@@ -59,7 +59,8 @@ struct DecodeParams {
   int cache_batch;
   const int* cache_leftpad;  // (B,)
   // Shared prefixes (decode_prefix_launch only): sequences [i * prefix_n, (i + 1) * prefix_n) share prefix i, whose
-  // valid rows are seqlens[i] (clamped to [0, s_cap]) of a (P, s_cap, Hkv, D) cache; the descales are (P, Hkv).
+  // valid rows are seqlens[i] (clamped to [0, s_cap]) of a (P, s_cap, Hkv, D) cache, or with a block table of the
+  // pages block_table[i * bt_stride + j] of a pool (the paged fields above, b = i); the descales are (P, Hkv).
   int prefix_n;
   // Tree attention (speculative decoding), with causal set; nullptr: none.  Byte u of row cu[b] + t (b * sq + t
   // uniform; row stride sq) is nonzero iff new token t of sequence b sees appended key u of its own call (u < n_b;
@@ -86,11 +87,13 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
 
 // The shared-prefix pass: attention of every query row to its group's prefix, into the partial slabs of `p.part`
 // (the same layout as decode_fwd_launch's; a caller merges both passes' slabs with one decode_combine_launch).  The
-// caches k_prefix / v_prefix are (n_prefix, p.s_cap, Hkv, D) with mergeable first two dimensions; p.seqlens are the
-// prefixes' valid rows, p.k_descale / p.v_descale (n_prefix, Hkv) with e4m3 caches, p.prefix_n = B / n_prefix.
-// Every prefix key is visible to every query token (p.n_new must be 0); q is rotated as in decode_fwd_launch (with
-// p.tree_mask, at the depth positions; the mask does not mask prefix keys).  No
-// append, block table, cache slots, left pads or e4m3 q.  The grid is (n_splits, decode_prefix_slots(p), n_prefix *
+// caches k_prefix / v_prefix are (n_prefix, p.s_cap, Hkv, D) with mergeable first two dimensions, or with
+// p.page_size set page pools (num_pages, page_size, Hkv, D) whose rows of prefix i are named by row i of p.block_table
+// (p.s_cap = max_prefix_blocks * page_size; the same page sizes, boxes and skipped pages as decode_fwd_launch's paged
+// cache); p.seqlens are the prefixes' valid rows, p.k_descale / p.v_descale (n_prefix, Hkv) with e4m3 caches,
+// p.prefix_n = B / n_prefix.  Every prefix key is visible to every query token (p.n_new must be 0); q is rotated as
+// in decode_fwd_launch (with p.tree_mask, at the depth positions; the mask does not mask prefix keys).  No append,
+// cache slots, left pads or e4m3 q.  The grid is (n_splits, decode_prefix_slots(p), n_prefix *
 // Hkv): a CTA takes 64 consecutive packed rows of one group, rows [b0 * sq, (b0 + n) * sq) of a uniform q or
 // [cu[b0], cu[b0 + n]) of a varlen one (b0 = prefix * n), each row (sequence, token, head-in-group) in that order.
 const char* decode_prefix_launch(int dtype, int cache_dtype, const TensorView& k_prefix, const TensorView& v_prefix,

@@ -62,7 +62,10 @@
 // sq) of a uniform q or [cu[b0], cu[b0 + n]) of a varlen one, so the group's samples share each prefix K / V tile.
 // Everything runs as a call with cache slot i, seqlens[i] valid rows, no append (every prefix key is visible to every
 // row) and descales [i, kv head]; only the rotary position and the lse address need a row's own sequence and token.
-// Its partials go to slabs after the suffix pass's, and the one combine merges both.
+// Its partials go to slabs after the suffix pass's, and the one combine merges both.  A paged prefix (page_size set)
+// is a pool of pages named by a (P, max_prefix_blocks) block table, P_cap = max_prefix_blocks * page_size: with b the
+// prefix, the paged producer indexes the table by prefix exactly as the suffix pass indexes it by sequence, so the pool
+// may be the suffix pass's own pool, with the prompt's pages in one table and each sample's pages in the other.
 #include <limits.h>
 #include <math_constants.h>
 
@@ -399,7 +402,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
   const int group = p.hq / p.hkv;
   int b, kv_head, row0;
   int2 qr;  // the sequence's first packed query row and token count (kPrefix: the group's)
-  if constexpr (kPrefix) {  // b is the prefix: it indexes seqlens, the cache slot and the descales
+  if constexpr (kPrefix) {  // b is the prefix: it indexes seqlens, the cache slot or block table, and the descales
     b = blockIdx.z / p.hkv;
     kv_head = blockIdx.z % p.hkv;
     qr = prefix_rows(p, b * p.prefix_n);
@@ -467,7 +470,7 @@ decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ 
 
   if (threadIdx.x >= kProducer) {
     // ------------------------------------------------------------------ TMA producer
-    if (!kPrefix && p.page_size != 0) {
+    if (p.page_size != 0) {
       if (n_tiles > 0)
         produce_paged<kD, kFp8, kQ8>(&tm_k, &tm_v, load_full, load_empty, smem_load, p, b, kv_head, j0, n_tiles,
                                      kmax);
@@ -964,6 +967,19 @@ __global__ void decode_combine_kernel(const float* parts, long long part_stride,
   if (lane == 0) lse_out[li] = lse;
 }
 
+// Rows per TMA box of a cache's tensor maps, or an error for a bad page size: a paged cache's maps cover the whole
+// pool and a box is at most one page; a contiguous cache takes one 128-key tile per box.
+const char* box_rows_of(const DecodeParams& p, int& box_rows) {
+  box_rows = kTile;
+  if (p.page_size == 0) return nullptr;
+  const bool size_ok = p.page_size == 16 || p.page_size == 32 || p.page_size == 64 ||
+                       (p.page_size > 0 && p.page_size % kTile == 0);
+  if (!size_ok) return "page_size must be 16, 32, 64 or a positive multiple of 128";
+  if (p.block_table == nullptr) return "a paged cache needs a block table";
+  if (p.page_size < kTile) box_rows = p.page_size;
+  return nullptr;
+}
+
 }  // namespace dec
 
 const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_cache, const TensorView& v_cache,
@@ -989,20 +1005,14 @@ const char* decode_fwd_launch(int dtype, int cache_dtype, const TensorView& k_ca
   if (p.tree_mask != nullptr && !p.causal) return "a tree mask replaces the causal rule: it needs causal";
   if (k_cache.row_stride != v_cache.row_stride || k_cache.head_stride != v_cache.head_stride)
     return "k_cache and v_cache must have the same strides";
-  if (p.page_size != 0) {
-    const bool size_ok = p.page_size == 16 || p.page_size == 32 || p.page_size == 64 ||
-                         (p.page_size > 0 && p.page_size % dec::kTile == 0);
-    if (!size_ok) return "page_size must be 16, 32, 64 or a positive multiple of 128";
-    if (p.block_table == nullptr) return "a paged cache needs a block table";
-  }
+  int box_rows;
+  if (const char* e = dec::box_rows_of(p, box_rows)) return e;
   if (p.rotary_cos != nullptr) {
     if (p.rotary_sin == nullptr || p.rotary_seqlens == nullptr) return "rotary needs cos, sin and rotary_seqlens";
     if (p.rotary_half <= 0 || p.rotary_half % 8 != 0 || 2 * p.rotary_half > head_dim)
       return "rotary_dim must be a positive multiple of 16, at most head_dim";
     if (p.seqlen_ro < 1) return "the rotary tables must have at least one row";
   }
-  // a paged cache's tensor maps cover the whole pool; a box is at most one page
-  const int box_rows = p.page_size != 0 && p.page_size < dec::kTile ? p.page_size : dec::kTile;
   // e4m3 rows are head_dim bytes: one 128-byte swizzle span at head_dim 128, one 64-byte span at 64
   const int elem_bytes = fp8 ? 1 : 2;
   const int swizzle = fp8 ? head_dim : 128;
@@ -1089,9 +1099,10 @@ const char* decode_prefix_launch(int dtype, int cache_dtype, const TensorView& k
   if (!fp8 && cache_dtype != dtype) return "the prefix caches must have q's dtype or be e4m3";
   if (fp8 != (p.k_descale != nullptr && p.v_descale != nullptr))
     return "e4m3 prefix caches need k / v descales, and only e4m3 caches take them";
-  if (p.q_descale != nullptr || p.n_new != 0 || p.page_size != 0 || p.cache_batch_idx != nullptr ||
-      p.cache_leftpad != nullptr)
-    return "the shared-prefix pass takes no q_descale, append, block table, cache slots or left pads";
+  if (p.q_descale != nullptr || p.n_new != 0 || p.cache_batch_idx != nullptr || p.cache_leftpad != nullptr)
+    return "the shared-prefix pass takes no q_descale, append, cache slots or left pads";
+  int box_rows;
+  if (const char* e = dec::box_rows_of(p, box_rows)) return e;
   if (p.hkv <= 0 || p.hq % p.hkv != 0) return "query heads must be a multiple of kv heads";
   if (p.tree_mask != nullptr && !p.causal) return "a tree mask replaces the causal rule: it needs causal";
   if (n_prefix < 1 || p.batch % n_prefix != 0 || p.prefix_n != p.batch / n_prefix)
@@ -1111,8 +1122,8 @@ const char* decode_prefix_launch(int dtype, int cache_dtype, const TensorView& k
   const int elem_bytes = fp8 ? 1 : 2;
   const int swizzle = fp8 ? head_dim : 128;
   CUtensorMap tk, tv;
-  if (const char* e = make_tensor_map(&tk, k_prefix, elem_bytes, dec::kTile, head_dim, swizzle)) return e;
-  if (const char* e = make_tensor_map(&tv, v_prefix, elem_bytes, dec::kTile, head_dim, swizzle)) return e;
+  if (const char* e = make_tensor_map(&tk, k_prefix, elem_bytes, box_rows, head_dim, swizzle)) return e;
+  if (const char* e = make_tensor_map(&tv, v_prefix, elem_bytes, box_rows, head_dim, swizzle)) return e;
   const dim3 grid(n_splits, static_cast<unsigned>(slots), n_prefix * p.hkv);
   cudaError_t err = cudaSuccess;
   auto launch = [&](auto kern, int smem, int threads) {

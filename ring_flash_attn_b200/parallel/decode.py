@@ -135,7 +135,8 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
                   cache_leftpad: Optional[Tensor] = None, prefix_k_cache: Optional[Tensor] = None,
                   prefix_v_cache: Optional[Tensor] = None, prefix_seqlens: Optional[Tensor] = None,
                   prefix_k_descale: Optional[Tensor] = None, prefix_v_descale: Optional[Tensor] = None,
-                  prefix_splits: Optional[int] = None, tree_mask: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+                  prefix_splits: Optional[int] = None, tree_mask: Optional[Tensor] = None,
+                  prefix_block_table: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
     """Local split-KV kernel (appending ``k`` / ``v`` first when given), then the combine over the splits and, for
     ``world > 1``, over the gathered per-rank partials.  ``splits`` overrides :func:`num_splits`.  With
     ``block_table`` the caches are page pools (see :func:`cp_flash_attn_with_kvcache`).  e4m3 caches take contiguous
@@ -149,7 +150,9 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
     ``prefix_k_cache`` / ``prefix_v_cache`` ``(P, P_cap, Hkv, D)`` (contiguous), ``prefix_seqlens`` ``(P,)`` int32 and,
     for e4m3 caches, contiguous fp32 ``(P, Hkv)`` ``prefix_k_descale`` / ``prefix_v_descale``, a second kernel adds
     the attention of sequence ``b`` to prefix ``b // (B // P)``, in ``prefix_splits`` (default
-    :func:`num_splits_prefix`) more partial slabs that the same combine merges.  ``tree_mask`` (contiguous bool
+    :func:`num_splits_prefix`) more partial slabs that the same combine merges; with ``prefix_block_table``
+    ``(P, max_prefix_blocks)`` int32 the prefix caches are page pools, as ``block_table`` makes the caches, and may be
+    the very tensors ``k_cache`` / ``v_cache``.  ``tree_mask`` (contiguous bool
     ``(B, Sq, Sq)``, or ``(total_q, max_seqlen_q)`` when varlen; needs ``causal``) says which appended keys each new
     token sees and sets the rotary positions of ``q`` and ``k`` (see :func:`cp_flash_attn_with_kvcache`); it is passed
     on every rank."""
@@ -175,10 +178,12 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
     prefix = prefix_k_cache is not None
     if prefix and prefix_splits is None:
         dev = q.device.index if q.device.index is not None else torch.cuda.current_device()
-        n_prefix, hkv = prefix_k_cache.shape[0], prefix_k_cache.shape[2]
+        n_prefix = prefix_k_cache.shape[0] if prefix_block_table is None else prefix_block_table.shape[0]
+        hkv = prefix_k_cache.shape[2]
         slots = prefix_tile_slots(b // n_prefix, max_seqlen_q if varlen else sq, hq, hkv,
                                   total_q if varlen else None)
-        prefix_splits = num_splits_prefix(n_prefix, slots, hkv, prefix_k_cache.shape[1], _sm_count(dev))
+        prefix_splits = num_splits_prefix(n_prefix, slots, hkv, _capacity(prefix_k_cache, prefix_block_table),
+                                          _sm_count(dev))
     n_slabs = splits + (prefix_splits if prefix else 0)
     n_out = rows_b * rows_sq * hq * d
     size = n_out + rows_b * hq * rows_sq
@@ -196,10 +201,12 @@ def kernel_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Te
                  rotary_seqlens, bool(rotary_interleaved), *extra)
     cuda_ext.note_launch(2 if k is not None else 1)
     if prefix:  # the prefix partials go to the slabs after the suffix pass's
+        pextra = () if tree_mask is None else (tree_mask,)
+        if prefix_block_table is not None:
+            pextra = (tree_mask, prefix_block_table)
         C.decode_prefix_fwd(q, prefix_k_cache, prefix_v_cache, prefix_seqlens, causal, softmax_scale, parts[splits:],
                             prefix_k_descale, prefix_v_descale, cu_seqlens_q, int(max_seqlen_q) if varlen else 0,
-                            rotary_cos, rotary_sin, rotary_seqlens, bool(rotary_interleaved),
-                            *(() if tree_mask is None else (tree_mask,)))
+                            rotary_cos, rotary_sin, rotary_seqlens, bool(rotary_interleaved), *pextra)
         cuda_ext.note_launch()
     if world > 1:
         mine = torch.empty(size, dtype=torch.float32, device=q.device)
@@ -328,16 +335,24 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
             raise ValueError(f"cache_batch_idx[{i}] = {slot} is outside the {n_pages}-slot cache")
         if not 0 <= lp <= lens[i]:
             raise ValueError(f"cache_leftpad[{i}] = {lp} is outside [0, cache_seqlens[{i}]] = [0, {lens[i]}]")
-    # shared prefixes (prefix_k, prefix_v, prefix_seqlens, prefix_k_descale, prefix_v_descale): sequence i reads
-    # rows [0, plens[i // n]) of prefix i // n ahead of its own keys
+    # shared prefixes (prefix_k, prefix_v, prefix_seqlens, prefix_k_descale, prefix_v_descale, prefix_block_table):
+    # sequence i reads rows [0, plens[i // n]) of prefix i // n ahead of its own keys
     plens = []
     if prefix is not None:
-        pk, pv, pseq, pkd, pvd = prefix
-        n_per = b // pk.shape[0]
+        pk, pv, pseq, pkd, pvd, ptable = prefix
+        n_per = b // pseq.shape[0]
+        p_cap = _capacity(pk, ptable)
         plens = pseq.tolist()
         for j, x in enumerate(plens):
-            if not 0 <= x <= pk.shape[1]:
-                raise ValueError(f"prefix_seqlens[{j}] = {x} is outside [0, P_cap] = [0, {pk.shape[1]}]")
+            if not 0 <= x <= p_cap:
+                raise ValueError(f"prefix_seqlens[{j}] = {x} is outside [0, P_cap] = [0, {p_cap}]")
+        if ptable is not None:  # the pages holding the visible rows, in table order, checked before any append
+            pps = pk.shape[1]
+            ppages = [row[:-(-n // pps)] for row, n in zip(ptable.tolist(), plens)]
+            for j, pages in enumerate(ppages):
+                if not all(0 <= x < pk.shape[0] for x in pages):
+                    raise ValueError(f"prefix_block_table[{j}] points outside the {pk.shape[0]}-page pool for a "
+                                     "page it reads")
     if k is not None:  # rows past the capacity (or whose page is outside the pool) are dropped, as in the kernel path
         if fp8 and k.dtype != torch.float8_e4m3fn:  # pre-quantised e4m3 k / v are stored as they are
             k = torch.cat([quantize_e4m3(k[lo:lo + n], k_descale[i]) for i, (lo, n) in enumerate(spans)])
@@ -375,7 +390,10 @@ def _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scal
             kk, vv = kk.float() * k_descale[i][:, None], vv.float() * v_descale[i][:, None]
         if n_pre:  # the prefix rows come first, and every query token sees them
             p = i // n_per
-            pkk, pvv = pk[p, :n_pre], pv[p, :n_pre]
+            if ptable is None:
+                pkk, pvv = pk[p, :n_pre], pv[p, :n_pre]
+            else:
+                pkk, pvv = pk[ppages[p]].flatten(0, 1)[:n_pre], pv[ppages[p]].flatten(0, 1)[:n_pre]
             if fp8:
                 pkk, pvv = pkk.float() * pkd[p][:, None], pvv.float() * pvd[p][:, None]
             kk, vv = torch.cat([pkk.to(kk.dtype), kk]), torch.cat([pvv.to(vv.dtype), vv])
@@ -415,7 +433,8 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
               cache_batch_idx: Optional[Tensor] = None, cache_leftpad: Optional[Tensor] = None,
               prefix_k_cache: Optional[Tensor] = None, prefix_v_cache: Optional[Tensor] = None,
               prefix_seqlens: Optional[Tensor] = None, prefix_k_descale: Optional[Tensor] = None,
-              prefix_v_descale: Optional[Tensor] = None, tree_mask: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
+              prefix_v_descale: Optional[Tensor] = None, tree_mask: Optional[Tensor] = None,
+              prefix_block_table: Optional[Tensor] = None) -> Tuple[Tensor, Tensor]:
     """q (B, Sq, Hq, D) -> (out (B, Sq, Hq, D) in q.dtype (bf16 for an e4m3 q), lse (B, Hq, Sq) fp32).  ``k`` /
     ``v`` are appended to the caches of rank ``append_rank`` only (-1: no append); ``group`` is the process group's
     name ("" = world); with ``block_table`` the caches are this rank's page pools; e4m3 caches come with contiguous
@@ -427,7 +446,9 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
     ``prefix_v_cache`` (P, P_cap, Hkv, D) with ``prefix_seqlens`` (P,) int32 (and fp32 (P, Hkv) descales for e4m3)
     are this rank's shards of the prefixes shared by consecutive groups of B / P sequences (read-only).  ``tree_mask``
     (B, Sq, Sq) bool, or (total_q, max_seqlen_q) when varlen, says which appended keys each new token sees; it is
-    passed on every rank, since it also sets the rotary positions of q."""
+    passed on every rank, since it also sets the rotary positions of q.  With ``prefix_block_table``
+    (P, max_prefix_blocks) int32 the prefix caches are a page pool, possibly ``k_cache`` / ``v_cache`` themselves: they
+    stay out of ``mutates_args`` because the op never writes them (appends land in the suffix's pages only)."""
     pg = resolve_group(group)
     rank, world = group_info(pg)
     if k is not None and not 0 <= append_rank < world:
@@ -443,10 +464,11 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
                              cache_batch_idx=cache_batch_idx, cache_leftpad=cache_leftpad,
                              prefix_k_cache=prefix_k_cache, prefix_v_cache=prefix_v_cache,
                              prefix_seqlens=prefix_seqlens, prefix_k_descale=prefix_k_descale,
-                             prefix_v_descale=prefix_v_descale, tree_mask=tree_mask)
+                             prefix_v_descale=prefix_v_descale, tree_mask=tree_mask,
+                             prefix_block_table=prefix_block_table)
     rotary = None if rotary_cos is None else (rotary_cos, rotary_sin, rotary_seqlens, rotary_interleaved)
     prefix = None if prefix_k_cache is None else (prefix_k_cache, prefix_v_cache, prefix_seqlens, prefix_k_descale,
-                                                  prefix_v_descale)
+                                                  prefix_v_descale, prefix_block_table)
     return _dense_decode(q, k_cache, v_cache, cache_seqlens, k, v, causal, softmax_scale, pg, world, block_table,
                          k_descale, v_descale, cu_seqlens_q, max_seqlen_q, rotary, q_descale, cache_batch_idx,
                          cache_leftpad, prefix, None if tree_mask is None else tree_mask.view(-1, tree_mask.shape[-1]))
@@ -456,7 +478,8 @@ def cp_decode(q: Tensor, k_cache: Tensor, v_cache: Tensor, cache_seqlens: Tensor
 def _(q, k_cache, v_cache, cache_seqlens, k, v, append_rank, softmax_scale, causal, group, block_table, k_descale,
       v_descale, cu_seqlens_q, max_seqlen_q, rotary_cos=None, rotary_sin=None, rotary_seqlens=None,
       rotary_interleaved=True, q_descale=None, cache_batch_idx=None, cache_leftpad=None, prefix_k_cache=None,
-      prefix_v_cache=None, prefix_seqlens=None, prefix_k_descale=None, prefix_v_descale=None, tree_mask=None):
+      prefix_v_cache=None, prefix_seqlens=None, prefix_k_descale=None, prefix_v_descale=None, tree_mask=None,
+      prefix_block_table=None):
     out = q.new_empty(q.shape, dtype=_out_dtype(q))
     if cu_seqlens_q is not None:
         total_q, hq, _ = q.shape
@@ -469,12 +492,12 @@ def _valid_page_size(ps: int) -> bool:
     return ps in (16, 32, 64) or (ps > 0 and ps % KEY_TILE == 0)
 
 
-def _check_block_table(q, k_cache, v_cache, block_table, b):
+def _check_block_table(q, k_cache, v_cache, block_table, b, name="block_table", rows="B", blocks="max_blocks"):
     if (block_table.dtype != torch.int32 or block_table.dim() != 2 or block_table.shape[0] != b
             or block_table.shape[1] < 1 or block_table.stride(1) != 1):
-        raise ValueError("block_table must be a (B, max_blocks) int32 tensor with stride(1) == 1")
+        raise ValueError(f"{name} must be a ({rows}, {blocks}) int32 tensor with stride(1) == 1")
     if block_table.device != q.device:
-        raise ValueError("block_table must be on q's device")
+        raise ValueError(f"{name} must be on q's device")
     n_blocks, ps = k_cache.shape[:2]
     if not _valid_page_size(ps):
         raise ValueError(f"page_size {ps} is not supported: use 16, 32, 64 or a positive multiple of 128")
@@ -482,7 +505,7 @@ def _check_block_table(q, k_cache, v_cache, block_table, b):
         if c.stride(0) != ps * c.stride(1) or c.stride(3) != 1:
             raise ValueError("the page pools must be mergeable: stride(0) == page_size * stride(1), stride(3) == 1")
     if n_blocks * ps >= 2 ** 31 or block_table.shape[1] * ps >= 2 ** 31:
-        raise ValueError("num_blocks * page_size and max_blocks * page_size must be below 2^31")
+        raise ValueError(f"num_blocks * page_size and {blocks} * page_size must be below 2^31")
 
 
 def _check_descale(name, x, q, b, hkv):
@@ -505,25 +528,36 @@ def _check_cache_index(name, x, q, b):
         raise ValueError(f"{name} must be on q's device")
 
 
-def _check_prefix(q, k_cache, pk, pv, pseq, pkd, pvd, b, hkv, d):
-    """Checks the shared prefixes and returns their descales as the contiguous (P, Hkv) fp32 tensors the kernels read
-    (None for bf16 / fp16 caches)."""
+def _check_prefix(q, k_cache, pk, pv, pseq, pkd, pvd, b, hkv, d, pbt=None):
+    """Checks the shared prefixes (a page pool with ``pbt``, the prefix block table) and returns their descales as
+    the contiguous (P, Hkv) fp32 tensors the kernels read (None for bf16 / fp16 caches)."""
     if pk is None or pv is None or pseq is None:
-        raise ValueError("pass prefix_k_cache, prefix_v_cache and prefix_seqlens together")
+        raise ValueError("pass prefix_k_cache, prefix_v_cache and prefix_seqlens together"
+                         + (" (prefix_block_table names pages of the prefix caches)" if pbt is not None else ""))
     if q.dtype == torch.float8_e4m3fn:
         raise ValueError("a shared prefix needs a bf16 / fp16 q: q_descale varies per sequence inside a packed prefix "
                          "tile, which fp8 (e4m3) queries with a prefix do not support")
+    paged = pbt is not None
     for name, x, c in (("prefix_k_cache", pk, k_cache), ("prefix_v_cache", pv, k_cache)):
-        if not isinstance(x, Tensor) or x.dim() != 4 or not x.is_contiguous():
-            raise ValueError(f"{name} must be a contiguous (P, P_cap, Hkv, D) tensor")
+        if not isinstance(x, Tensor) or x.dim() != 4 or not (paged or x.is_contiguous()):
+            raise ValueError(f"{name} must be a (num_blocks, page_size, Hkv, D) page pool with prefix_block_table"
+                             if paged else f"{name} must be a contiguous (P, P_cap, Hkv, D) tensor")
         if x.dtype != c.dtype:
             raise ValueError(f"{name} must have the cache's dtype ({c.dtype}), not {x.dtype}")
     if pk.shape != pv.shape or tuple(pk.shape[2:]) != (hkv, d):
         raise ValueError(f"prefix_k_cache {tuple(pk.shape)} and prefix_v_cache {tuple(pv.shape)} must both be "
-                         f"(P, P_cap, Hkv, D) with (Hkv, D) = {(hkv, d)}")
-    n_prefix, p_cap = pk.shape[:2]
-    if n_prefix < 1 or p_cap < 1 or n_prefix * p_cap >= 2 ** 31:
-        raise ValueError(f"prefix caches: P = {n_prefix} and P_cap = {p_cap} must be >= 1 with P * P_cap < 2^31")
+                         f"{'(num_blocks, page_size' if paged else '(P, P_cap'}, Hkv, D) with (Hkv, D) = {(hkv, d)}")
+    if paged:
+        if not isinstance(pbt, Tensor) or pbt.dim() != 2 or pbt.shape[0] < 1:
+            raise ValueError("prefix_block_table must be a (P, max_prefix_blocks) int32 tensor with stride(1) == 1")
+        _check_block_table(q, pk, pv, pbt, pbt.shape[0], "prefix_block_table", "P", "max_prefix_blocks")
+        if pk.stride() != pv.stride():
+            raise ValueError("the prefix page pools must have the same strides")
+        n_prefix, p_cap = pbt.shape[0], _capacity(pk, pbt)
+    else:
+        n_prefix, p_cap = pk.shape[:2]
+        if n_prefix < 1 or p_cap < 1 or n_prefix * p_cap >= 2 ** 31:
+            raise ValueError(f"prefix caches: P = {n_prefix} and P_cap = {p_cap} must be >= 1 with P * P_cap < 2^31")
     if pk.device != q.device or pv.device != q.device:
         raise ValueError("prefix_k_cache / prefix_v_cache must be on q's device")
     if b % n_prefix != 0:
@@ -609,7 +643,8 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
                                max_seqlen_q=None, rotary_cos=None, rotary_sin=None, rotary_interleaved=True,
                                rotary_seqlens=None, window_size=(-1, -1), alibi_slopes=None, q_descale=None,
                                cache_batch_idx=None, cache_leftpad=None, prefix_k_cache=None, prefix_v_cache=None,
-                               prefix_seqlens=None, prefix_k_descale=None, prefix_v_descale=None, tree_mask=None):
+                               prefix_seqlens=None, prefix_k_descale=None, prefix_v_descale=None, tree_mask=None,
+                               prefix_block_table=None):
     """Decode attention of new query tokens against a KV cache sharded over ``group`` (modelled on flash-attn's
     ``flash_attn_with_kvcache``).  Inference only: no gradient.
 
@@ -681,8 +716,23 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
       only and clamped to ``[0, P_cap]`` (a CUDA graph replay uses its current contents); the dense path raises
       ``ValueError`` for a value outside that range.  Missing pieces, shape / dtype / device / contiguity mismatches,
       ``B % P != 0`` and an e4m3 ``q`` with a prefix (``q_descale`` would vary inside a packed prefix tile) raise
-      ``ValueError``.  Paged prefixes, prefixes shared by non-consecutive sequences and nested prefixes are not
-      supported.
+      ``ValueError``.  Prefixes shared by non-consecutive sequences and nested prefixes are not supported.
+    * Paged prefixes: ``prefix_block_table`` ``(P, max_prefix_blocks)`` int32 on q's device (``stride(1) == 1``),
+      optional, follows the rules of ``block_table``.  ``prefix_k_cache`` / ``prefix_v_cache`` are then this rank's
+      page pool ``(num_blocks, page_size, Hkv, D)``, with ``stride(0) == page_size * stride(1)``, in the dtype of
+      ``k_cache``; ``page_size`` is 16, 32, 64 or a positive multiple of 128, and ``num_blocks * page_size < 2**31``.
+      Row ``j`` of prefix ``p`` lives at row ``j % page_size`` of page ``prefix_block_table[p, j // page_size]``.
+      ``P`` is ``prefix_block_table.shape[0]`` and ``P_cap`` is ``max_prefix_blocks * page_size``; ``prefix_seqlens``
+      and the prefix descales keep their shapes.  The pool may be the very tensors ``k_cache`` / ``v_cache`` of a
+      paged call (one pool per rank, the prompt's pages named in ``prefix_block_table`` and each sample's own pages
+      in ``block_table``, as paged serving engines keep them), or a pool of its own beside a contiguous suffix cache,
+      with or without ``cache_batch_idx`` / ``cache_leftpad``.  Appends go to the suffix only, before either pass
+      reads; a sample whose appended rows land in a page of its prompt is a caller error (the prompt's rows are then
+      overwritten).  Entries of pages that hold no visible prefix row are never read (-1 is fine).  An entry outside
+      the pool for a page that is read gives an undefined result on the kernel path, but no access outside the pool;
+      the dense path raises ``ValueError``.  The kernel path reads the table on the device only (a CUDA graph replay
+      uses its current contents).  The result is bitwise that of the contiguous prefix call on the same rows at equal
+      ``P_cap`` and split counts.
     * ``k`` / ``v`` ``(B, Sq, Hkv, D)``, optional, the same on every rank: written in place into the caches of rank
       ``append_rank`` only, at rows ``[cache_seqlens[b], cache_seqlens[b] + Sq)``, before attention (rows past
       ``S_cap`` are dropped).  The caller advances ``cache_seqlens``.  ``append_rank`` is required with ``k`` / ``v``
@@ -844,10 +894,12 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
                 raise ValueError(f"k / v must be (B, Sq, Hkv, D) = {(b, sq, hkv, d)} in q's dtype")
     elif append_rank is not None:
         raise ValueError("append_rank must be None when no k / v are given")
-    has_prefix = prefix_k_cache is not None or prefix_v_cache is not None or prefix_seqlens is not None
+    has_prefix = (prefix_k_cache is not None or prefix_v_cache is not None or prefix_seqlens is not None
+                  or prefix_block_table is not None)
     if has_prefix:
         prefix_k_descale, prefix_v_descale = _check_prefix(q, k_cache, prefix_k_cache, prefix_v_cache, prefix_seqlens,
-                                                           prefix_k_descale, prefix_v_descale, b, hkv, d)
+                                                           prefix_k_descale, prefix_v_descale, b, hkv, d,
+                                                           prefix_block_table)
     elif prefix_k_descale is not None or prefix_v_descale is not None:
         raise ValueError("prefix_k_descale / prefix_v_descale are only taken with prefix_k_cache / prefix_v_cache")
     if rotary_cos is not None or rotary_sin is not None:
@@ -870,5 +922,6 @@ def cp_flash_attn_with_kvcache(q, k_cache, v_cache, cache_seqlens, k=None, v=Non
                          scale, bool(causal), group_name(group), block_table, k_descale, v_descale, cu_seqlens_q,
                          max_seqlen_q if varlen else 0, rotary_cos, rotary_sin, rotary_seqlens,
                          bool(rotary_interleaved), q_descale, cache_batch_idx, cache_leftpad, prefix_k_cache,
-                         prefix_v_cache, prefix_seqlens, prefix_k_descale, prefix_v_descale, tree_mask)
+                         prefix_v_cache, prefix_seqlens, prefix_k_descale, prefix_v_descale, tree_mask,
+                         prefix_block_table)
     return (out, lse) if return_softmax_lse else out
