@@ -396,9 +396,11 @@ def run_forward(geom: dict, d: int, dtype, window: bool, regime: str, device, se
     assert_lse(f"{tag}: lse", lse[:, rows], l64[:, rows], llp[:, rows], row_ids=rows, report="lse")
 
 
-def run_backward(geom: dict, d: int, dtype, window: bool, regime: str, device, dkv_dtype=torch.float32, seed: int = 0):
+def run_backward(geom: dict, d: int, dtype, window: bool, regime: str, device, dkv_dtype=torch.float32, seed: int = 0,
+                 deterministic: bool = False):
     """lse and delta come from the fp64 oracle, so the backward is tested apart from the forward.  ``dkv_dtype``:
-    fp32 (the per-source transports) or the model dtype (world size 1 / the fused path)."""
+    fp32 (the per-source transports) or the model dtype (world size 1 / the fused path).  ``deterministic``: the
+    ordered launch groups of ``deterministic=True``.  Returns the kernels' (dq, dk, dv)."""
     plan = build_plan(geom, window)
     q, k, v, do = make_inputs(geom, d, dtype, regime, device, seed)
     scale = d ** -0.5
@@ -408,7 +410,7 @@ def run_backward(geom: dict, d: int, dtype, window: bool, regime: str, device, d
     dq = torch.zeros(q.shape, dtype=torch.float32, device=device)
     dk = torch.zeros(k.shape, dtype=dkv_dtype, device=device)
     dv = torch.zeros(v.shape, dtype=dkv_dtype, device=device)
-    attn_cuda.segments_backward(plan, plan.segments, do, q, k, v, lse32, delta32, scale, dq, dk, dv)
+    attn_cuda.segments_backward(plan, plan.segments, do, q, k, v, lse32, delta32, scale, dq, dk, dv, deterministic)
     g64 = plan_backward(plan, plan.segments, q, k, v, do, l64, delta64, scale)
     glp = plan_backward(plan, plan.segments, q, k, v, do, lse32, delta32, scale, mm_dtype=dtype, dkv_dtype=dkv_dtype)
     rows = chunk_rows(plan, device)
@@ -420,6 +422,7 @@ def run_backward(geom: dict, d: int, dtype, window: bool, regime: str, device, d
     assert_accurate(f"{tag}: dq", dq[rows], g64[0][rows], glp[0][rows], row_ids=rows, factor=f, report=key)
     assert_accurate(f"{tag}: dk", dk, g64[1], glp[1], factor=f, report=key)
     assert_accurate(f"{tag}: dv", dv, g64[2], glp[2], factor=f, report=key)
+    return dq, dk, dv
 
 
 def _poison(x: torch.Tensor, idx: torch.Tensor):
