@@ -252,14 +252,16 @@ def references(case: Case, plans, q, k, v, dout, transport: str, ranks: Optional
 
 
 def check(name: str, got: dict, ref64: dict, reflp: dict, report: str, factor: Optional[float] = None,
-          lse_rel: Optional[float] = None) -> None:
-    """Every output in ``got`` (token-major out / dq / dk / dv, lse (Hq, T)) within the precision-matched bound."""
+          lse_rel: Optional[float] = None, per_block: bool = False) -> None:
+    """Every output in ``got`` (token-major out / dq / dk / dv, lse (Hq, T)) within the precision-matched bound
+    (``per_block``: within every ``kernel_oracle.work_units`` block too)."""
     for key, val in got.items():
         if key == "lse":
             KO.assert_lse(f"{name}: lse", val, ref64["lse"], reflp["lse"], report="lse " + report, rel_limit=lse_rel)
         else:
             assert val.dtype == reflp[key].dtype, (name, key, val.dtype, reflp[key].dtype)
-            KO.assert_accurate(f"{name}: {key}", val, ref64[key], reflp[key], factor=factor, report=report)
+            KO.assert_accurate(f"{name}: {key}", val, ref64[key], reflp[key], factor=factor, report=report,
+                               **(KO.work_units(key) if per_block else {}))
 
 
 def report_key(transport: str, world: int) -> str:

@@ -244,18 +244,23 @@ def _layout(case: Case, kc: torch.Tensor, vc: torch.Tensor, lens, seed: int):
 
 
 def build_inputs(case: Case, dtype, d: int, regime: str, device, seed: int = 0,
-                 cache_seed: Optional[int] = None) -> Inputs:
-    """Seeded inputs (drawn on the CPU, so the same on every device).  q / k / v come from ``seed``, the cache from
-    ``cache_seed`` (default ``seed + 1``), so ranks can share the new tokens and hold different shards.  Regimes:
+                 cache_seed: Optional[int] = None, draw="cpu") -> Inputs:
+    """Seeded inputs, drawn on ``draw``: the CPU by default, so the same on every device; ``draw=device`` for caches
+    of gigabytes.  q / k / v come from ``seed``, the cache from ``cache_seed`` (default ``seed + 1``), so ranks can
+    share the new tokens and hold different shards.  Regimes:
     ``randn``; ``peaked`` (logits span about +-30 and rise with the key position, so a row's maximum is its last
     visible key) and ``peaked_reverse`` (key 0); ``large`` (|q|, |k| about 30); ``v_offset`` (V = 50 + randn)."""
     b, hq, hkv, s_cap = case.b, case.hq, case.hkv, case.s_cap
     smax = max(max(case.counts), 1)
-    gq = torch.Generator().manual_seed(seed)
-    gc = torch.Generator().manual_seed(seed + 1 if cache_seed is None else cache_seed)
-    q4 = torch.randn(b, smax, hq, d, generator=gq)
-    kn4, vn4 = torch.randn(b, smax, hkv, d, generator=gq), torch.randn(b, smax, hkv, d, generator=gq)
-    kc, vc = torch.randn(b, s_cap, hkv, d, generator=gc), torch.randn(b, s_cap, hkv, d, generator=gc)
+    gq = torch.Generator(device=draw).manual_seed(seed)
+    gc = torch.Generator(device=draw).manual_seed(seed + 1 if cache_seed is None else cache_seed)
+
+    def rn(*shape, g):
+        return torch.randn(shape, generator=g, device=draw)
+
+    q4 = rn(b, smax, hq, d, g=gq)
+    kn4, vn4 = rn(b, smax, hkv, d, g=gq), rn(b, smax, hkv, d, g=gq)
+    kc, vc = rn(b, s_cap, hkv, d, g=gc), rn(b, s_cap, hkv, d, g=gc)
     lens = [min(max(int(s), 0), s_cap) for s in case.seqlens]
     if regime in ("peaked", "peaked_reverse"):
         rev = regime == "peaked_reverse"
@@ -263,8 +268,8 @@ def build_inputs(case: Case, dtype, d: int, regime: str, device, seed: int = 0,
         q4 = 1.0 + 0.1 * q4
         for i, (n, c) in enumerate(zip(lens, case.counts)):
             vis = min(n + (c if case.append else 0), s_cap)
-            kc[i] = amp * _ramp(vis, torch.arange(s_cap), rev).view(-1, 1, 1) + 0.1 * kc[i]
-            kn4[i] = amp * _ramp(vis, n + torch.arange(smax), rev).view(-1, 1, 1) + 0.1 * kn4[i]
+            kc[i] = amp * _ramp(vis, torch.arange(s_cap, device=draw), rev).view(-1, 1, 1) + 0.1 * kc[i]
+            kn4[i] = amp * _ramp(vis, n + torch.arange(smax, device=draw), rev).view(-1, 1, 1) + 0.1 * kn4[i]
     elif regime == "large":
         q4, kn4, kc = (30.0 * x.sign() + x for x in (q4, kn4, kc))
     elif regime == "v_offset":
@@ -273,7 +278,7 @@ def build_inputs(case: Case, dtype, d: int, regime: str, device, seed: int = 0,
         raise ValueError(regime)
     fp8 = case.fp8
     if fp8 and case.saturate:  # +-1000: past 448 * descale for every descale here
-        sign = torch.ones(smax, hkv)
+        sign = torch.ones(smax, hkv, device=draw)
         sign[1::2] = -1.0
         kn4[..., 3] = 1000.0 * sign
         vn4[..., 5] = -1000.0 * sign
@@ -284,7 +289,7 @@ def build_inputs(case: Case, dtype, d: int, regime: str, device, seed: int = 0,
     q, k_new, v_new = (pack(x, case.counts).to(device) for x in (q4, kn4, vn4))
     kd = vd = None
     if fp8:
-        kd, vd = descales(b, hkv, "k", "cpu"), descales(b, hkv, "v", "cpu")
+        kd, vd = descales(b, hkv, "k", draw), descales(b, hkv, "v", draw)
         kc = torch.stack([dec.quantize_e4m3(kc[i], kd[i]) for i in range(b)])
         vc = torch.stack([dec.quantize_e4m3(vc[i], vd[i]) for i in range(b)])
         kd, vd = kd.to(device), vd.to(device)
@@ -491,9 +496,16 @@ def expected_caches(inp: Inputs, k0: torch.Tensor, v0: torch.Tensor, with_append
             appended(v0, inp.table, case.seqlens, inp.stored_v, case.counts))
 
 
-def run_decode(case: Case, dtype, d: int, regime: str, device, seed: int = 0):
-    """One case through ``kernel_decode`` against both references, then the cache bytes."""
-    inp = build_inputs(case, dtype, d, regime, device, seed)
+def sequence_blocks(case: Case):
+    """``assert_accurate`` blocks of a uniform call's packed (rows, Hq, D) out: one per (sequence, kv head)."""
+    assert not case.varlen
+    return (case.counts[0], case.group, None)
+
+
+def run_decode(case: Case, dtype, d: int, regime: str, device, seed: int = 0, draw="cpu", per_block: bool = False):
+    """One case through ``kernel_decode`` against both references, then the cache bytes.  ``per_block`` (a uniform
+    case): the bound also holds within every (sequence, kv head), the kernel's unit of work."""
+    inp = build_inputs(case, dtype, d, regime, device, seed, draw=draw)
     n_splits = case.splits if case.splits is not None else default_splits(case, device)
     k0, v0 = inp.k_cache.clone(), inp.v_cache.clone()
     q, k, v = call_views(inp, case.append)
@@ -506,7 +518,8 @@ def run_decode(case: Case, dtype, d: int, regime: str, device, seed: int = 0):
     assert out.dtype == dtype and out.shape == q.shape, (tag, out.dtype, out.shape)
     got_o, got_l = packed(case, out, lse)
     KO.assert_accurate(f"{tag}: out", got_o, o64, o32.to(dtype), factor=KO._factor(regime),
-                       report=report_key(dtype, d, case.fp8, regime))
+                       report=report_key(dtype, d, case.fp8, regime),
+                       blocks=sequence_blocks(case) if per_block else None)
     KO.assert_lse(f"{tag}: lse", got_l, l64, l32, report=f"decode lse {'e4m3' if case.fp8 else 'native'}")
     want_k, want_v = expected_caches(inp, k0, v0, case.append)
     for name, got, want in (("k_cache", inp.k_cache, want_k), ("v_cache", inp.v_cache, want_v)):

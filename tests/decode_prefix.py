@@ -45,18 +45,19 @@ class Prefix:
         return kw
 
 
-def make_prefix(case: DO.Case, dtype, d: int, device, lens: List[int], p_cap: int, seed: int = 7) -> Prefix:
-    """Seeded prefix shards (drawn on the CPU): ``len(lens)`` prefixes of ``p_cap`` rows, NaN past ``lens``; with an
-    e4m3 case, quantised with their own descales."""
-    g = torch.Generator().manual_seed(seed)
+def make_prefix(case: DO.Case, dtype, d: int, device, lens: List[int], p_cap: int, seed: int = 7,
+                draw="cpu") -> Prefix:
+    """Seeded prefix shards (drawn on ``draw``, the CPU by default): ``len(lens)`` prefixes of ``p_cap`` rows, NaN
+    past ``lens``; with an e4m3 case, quantised with their own descales."""
+    g = torch.Generator(device=draw).manual_seed(seed)
     n_prefix, hkv = len(lens), case.hkv
-    k, v = (torch.randn(n_prefix, p_cap, hkv, d, generator=g) for _ in range(2))
+    k, v = (torch.randn(n_prefix, p_cap, hkv, d, generator=g, device=draw) for _ in range(2))
     for i, n in enumerate(lens):
         k[i, n:] = float("nan")
         v[i, n:] = float("nan")
     kd = vd = None
     if case.fp8:
-        kd, vd = 1.3 * DO.descales(n_prefix, hkv, "k", "cpu"), 0.8 * DO.descales(n_prefix, hkv, "v", "cpu")
+        kd, vd = 1.3 * DO.descales(n_prefix, hkv, "k", draw), 0.8 * DO.descales(n_prefix, hkv, "v", draw)
         k = torch.stack([dec.quantize_e4m3(k[i], kd[i]) for i in range(n_prefix)])
         v = torch.stack([dec.quantize_e4m3(v[i], vd[i]) for i in range(n_prefix)])
         kd, vd = kd.to(device), vd.to(device)

@@ -39,6 +39,12 @@ class FakeExt:
     def _group_sum(self, x, hkv, rep):  # dK / dV of a kv head: sum over its query heads
         return x.view(x.shape[0], hkv, rep, x.shape[2]).sum(2)
 
+    def _accumulate(self, acc, x, dtype):  # a key tile's dK / dV after one more query segment
+        return acc + x
+
+    def _dq_part(self, x, q_row0, kv_row0):  # the dQ contribution of one key tile to rows q_row0 ..
+        return x
+
     # ------------------------------------------------------------------ forward
     def _fwd(self, q, k, v, items, segs, seg_lo, out, lse, scale, sqk=None, sv=None):
         hq, hkv = q.shape[1], k.shape[1]
@@ -116,11 +122,12 @@ class FakeExt:
                 lr = lse[:, rows]
                 p = torch.exp(s - torch.where(torch.isinf(lr), torch.full_like(lr, float("inf")), lr).unsqueeze(-1))
                 p = p.masked_fill(~m.unsqueeze(0), 0.0)
-                dv_t += torch.einsum("hnk,nhd->khd", self._p_for_pv(p, q.dtype), dof[rows])
+                dv_t = self._accumulate(dv_t, torch.einsum("hnk,nhd->khd", self._p_for_pv(p, q.dtype), dof[rows]),
+                                        q.dtype)
                 dp = torch.einsum("nhd,khd->hnk", dof[rows], vt)
                 ds = p * (dp - delta[:, rows].unsqueeze(-1)) * scale
-                dk_t += torch.einsum("hnk,nhd->khd", ds, qf[rows])
-                dq[rows] += torch.einsum("hnk,khd->nhd", ds, kt)
+                dk_t = self._accumulate(dk_t, torch.einsum("hnk,nhd->khd", ds, qf[rows]), q.dtype)
+                dq[rows] += self._dq_part(torch.einsum("hnk,khd->nhd", ds, kt), q_row0, kv_row0)
             dk[kv_row0:kv_row0 + kv_rows] = self._group_sum(dk_t, hkv, rep)  # written, not accumulated
             dv[kv_row0:kv_row0 + kv_rows] = self._group_sum(dv_t, hkv, rep)
 
